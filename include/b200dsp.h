@@ -68,6 +68,21 @@ extern "C" {
                                   * RationalResampler to 5 kS/s (broadcast_fm.h:52-53,165-170,196-202); output = complex_t at 5 kS/s, what
                                   * decoder_modules/radio/src/rds_demod.h consumes */
 #define B200_DEMOD_WFM_STEREO 7  /* demod::BroadcastFM stereo branch: pilot filter + PLL + L-R recovery -- broadcast_fm.h:147-190 */
+#define B200_DEMOD_WFM_RDS_BITS 9  /* the B200_DEMOD_WFM_RDS chain followed by RDSDemod (decoder_modules/radio/src/rds_demod.h:64-73, the
+                                    * b200_rds_demod_* block below) inside the front end: output = one b200_rds_symbol per recovered
+                                    * symbol.  The symbol count depends on the recovered clock: vfo_count of such a VFO is filled by
+                                    * b200_fe_wait (b200_fe_process, b200_shard_wait), valid when it returns like the data, so the
+                                    * b200_outputs given to b200_fe_submit must stay alive until that wait.  vfo_cap counts records and
+                                    * b200_fe_vfo_max_out bounds them (b200_rds_demod_max_out of the 5 kS/s samples); records past
+                                    * vfo_count are unspecified.  AF chain, volume and audio fields are ignored as for mode 8; the IF
+                                    * chain (blanker, squelch, FM IF noise reduction) applies as for mode 8. */
+
+/* one recovered RDS symbol: RDSDemod::soft and the differentially decoded bit of RDSDemod::out (0 or 1); 8 bytes, the element
+ * size of every other VFO output (complex_t, stereo_t) */
+typedef struct {
+    float    soft;
+    uint32_t bit;
+} b200_rds_symbol;
 
 #define B200_AGC_CARRIER 0   /* demod::AM::AGCMode (am.h:14-17) */
 #define B200_AGC_AUDIO   1
@@ -167,10 +182,10 @@ typedef struct {
 } b200_vfo_cfg;
 
 typedef struct {
-    /* per VFO: caller buffer for this chunk's output (stereo_t pairs, or complex_t for RAW) */
+    /* per VFO: caller buffer for this chunk's output (stereo_t pairs, complex_t for RAW / WFM_RDS, b200_rds_symbol for WFM_RDS_BITS) */
     void* vfo_out[B200_MAX_VFOS];
     int   vfo_cap[B200_MAX_VFOS];     /* capacity in output samples                               */
-    int   vfo_count[B200_MAX_VFOS];   /* OUT: samples produced this chunk                         */
+    int   vfo_count[B200_MAX_VFOS];   /* OUT: samples produced this chunk (WFM_RDS_BITS: set by b200_fe_wait) */
     /* FFT branch: dB lines completed during this chunk, fft_size floats each                     */
     float* fft_out;
     int   fft_cap_lines;
@@ -325,8 +340,9 @@ void b200_block_destroy(b200_block* b);
  * polyphase interpolator) -> slicer -> differential decoder.  Input: the complex 5 kS/s stream BroadcastFM's rdsOut carries
  * (b200_wfm_rds_create, or a front-end VFO in B200_DEMOD_WFM_RDS mode); `in` may be a host or a device pointer.  Per recovered
  * symbol one soft value (RDSDemod::soft) and one decoded bit (RDSDemod::out), written to HOST buffers of at least
- * b200_rds_demod_max_out(count) entries; returns the number of symbols of this call (it depends on the recovered clock, which
- * is why this block is not a front-end stage: every other count is known on the host before the launch).
+ * b200_rds_demod_max_out(count) entries; returns the number of symbols of this call (it depends on the recovered clock, so this
+ * call waits for its launch; a front-end VFO in B200_DEMOD_WFM_RDS_BITS mode runs the same kernel inside the submit / wait
+ * pipeline instead).
  * The three feedback loops run on one thread of the device in the reference's fp32 statement order; the band-pass in parallel. */
 typedef struct b200_rds_demod b200_rds_demod;
 b200_rds_demod* b200_rds_demod_create(void);

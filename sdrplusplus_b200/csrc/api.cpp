@@ -154,6 +154,66 @@ struct FftCore {
     }
 };
 
+// ------------------------------------------------------------------ RDSDemod (decoder_modules/radio/src/rds_demod.h)
+// One stream's carried state and tables, owned by a b200_rds_demod block or by a front-end VFO in B200_DEMOD_WFM_RDS_BITS mode.
+static_assert(sizeof(b200_rds_symbol) == 8 && sizeof(RdsSym) == sizeof(b200_rds_symbol), "one RDS symbol record is 8 bytes");
+struct RdsCore {
+    DevBuf state, taps, bank;
+    RdsState init;               // what reset() restores
+    RdsJob proto;                // coefficients and tables; job() fills in the rest per launch
+    int create(cudaStream_t s);
+    int reset(cudaStream_t s);
+    RdsJob job(const float2* in, int n, RdsSym* out, int out_cap, int* count) const {
+        RdsJob J = proto;
+        J.in = in; J.n = n; J.out = out; J.out_cap = out_cap; J.count = count;
+        return J;
+    }
+};
+int RdsCore::create(cudaStream_t s) {
+    // init() of rds_demod.h:20-41
+    const std::vector<float> bp = bandpass_c_taps(0.0, 2375.0, 100.0, 5000.0, false);      // (re, im) pairs
+    const std::vector<float> bk = mm_interp_bank(RDS_MM_PHASES, RDS_MM_TAPS);
+    const int nt = (int)bp.size() / 2;
+    if (nt < 2 || nt > RDS_MAXTAPS) { set_error("RDS band-pass of %d taps", nt); return B200_EINVAL; }
+    int rc;
+    if ((rc = state.alloc(sizeof(RdsState), false)) || (rc = taps.alloc(bp.size() * sizeof(float), false)) ||
+        (rc = bank.alloc(bk.size() * sizeof(float), false))) { return rc; }
+    RdsJob& J = proto;
+    memset(&J, 0, sizeof(J));
+    J.state = state.as<RdsState>(); J.taps = taps.as<float2>(); J.bank = bank.as<float>();
+    J.ntaps = nt;
+    J.set_point = (float)1.0; J.max_gain = (float)1e6; J.rate = (float)0.1;               // agc.init(NULL, 1.0, 1e6, 0.1)
+    pll_coefficients(0.005f, J.c1_alpha, J.c1_beta);                                       // costas.init(NULL, 0.005f)
+    J.c1_min = -3.1415926535f; J.c1_max = 3.1415926535f;                                   // FL_M_PI (math/constants.h:4)
+    const double baud = hz_to_rads(2375.0 / 2.0, 5000.0);
+    pll_coefficients(0.01, J.c2_alpha, J.c2_beta);                                         // costas2.init(NULL, 0.01, 0, f, f - 10 %, f + 10 %)
+    J.c2_min = (float)(baud - (baud * 0.1)); J.c2_max = (float)(baud + (baud * 0.1));
+    const double omega = 5000.0 / (2375.0 / 2.0);                                          // recov.init(NULL, omega, 1e-6, 0.01, 0.01)
+    J.mm_alpha = (float)0.01; J.mm_beta = (float)1e-6;
+    J.mm_min = (float)(omega * (1.0 - 0.01)); J.mm_max = (float)(omega * (1.0 + 0.01));
+    memset(&init, 0, sizeof(init));
+    init.gain = (float)1.0;
+    init.c2_freq = (float)baud;
+    init.mm_freq = (float)omega;
+    cudaError_t e = cudaMemcpyAsync(taps.p, bp.data(), bp.size() * sizeof(float), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) { e = cudaMemcpyAsync(bank.p, bk.data(), bk.size() * sizeof(float), cudaMemcpyHostToDevice, s); }
+    if (e == cudaSuccess) { e = cudaMemcpyAsync(state.p, &init, sizeof(RdsState), cudaMemcpyHostToDevice, s); }
+    if (e == cudaSuccess) { e = cudaStreamSynchronize(s); }
+    if (e != cudaSuccess) { return cuda_fail(e, "RDS demodulator tables"); }
+    return 0;
+}
+int RdsCore::reset(cudaStream_t s) {
+    // RDSDemod::reset (rds_demod.h:52-62): gain, loop phases / frequencies, band-pass delay line, MM offset / phase / lastOut,
+    // decoder memory.  MM::reset (mm.h:83-92) leaves its work-buffer tail alone: so does this.
+    RdsState cur, st = init;
+    B200_CK(cudaMemcpyAsync(&cur, state.p, sizeof(RdsState), cudaMemcpyDeviceToHost, s));
+    B200_CK(cudaStreamSynchronize(s));
+    memcpy(st.m_hist, cur.m_hist, sizeof(st.m_hist));
+    B200_CK(cudaMemcpyAsync(state.p, &st, sizeof(RdsState), cudaMemcpyHostToDevice, s));
+    B200_CK(cudaStreamSynchronize(s));
+    return 0;
+}
+
 // ------------------------------------------------------------------ front end
 struct VfoSlot {
     bool used = false;
@@ -161,6 +221,9 @@ struct VfoSlot {
     Chain chain;
     bool pend_offset = false, pend_bw = false;
     double new_offset = 0, new_bw = 0;
+    // B200_DEMOD_WFM_RDS_BITS: RDSDemod behind the chain, and where its records wait for the copy to a host buffer
+    std::unique_ptr<RdsCore> rds;
+    DevBuf rds_rec;
 };
 
 // input slots / event sets of a front end: a chunk uses slot (index % FE_SLOTS); up to FE_SLOTS chunks may be between submit and
@@ -208,6 +271,12 @@ struct b200_fe {
     DevBuf pp[FE_SLOTS];         // chunk after DC blocker / conjugate (one per chunk in flight)
     DevBuf dc_state, dc_segA, dc_segB;
     int max_eff = 0;             // largest chunk behind the decimator
+    // RDS symbol counts (B200_DEMOD_WFM_RDS_BITS VFOs): the device knows them only after the launch.  The kernel writes them
+    // into the row of the chunk's slot in pinned memory, in stream order before ev_out; b200_fe_wait reads them after it.
+    int* rds_count = nullptr;                // [FE_SLOTS][B200_MAX_VFOS], allocated with the first such VFO
+    struct RdsPend { int id, n_in, bound; };
+    std::vector<RdsPend> rds_pend[FE_SLOTS];
+    b200_outputs* rds_out[FE_SLOTS] = {};    // whose vfo_count b200_fe_wait fills
 };
 
 // (float)x * scale for the integer input formats: 1/32768 and 1/128 unless the caller set the scale of a
@@ -299,6 +368,7 @@ extern "C" void b200_fe_destroy(b200_fe* fe) {
     if (fe->own_stream) { cudaStreamDestroy(fe->own_stream); }
     if (fe->copy_stream) { cudaStreamDestroy(fe->copy_stream); }
     if (fe->fft_stream) { cudaStreamDestroy(fe->fft_stream); }
+    if (fe->rds_count) { cudaFreeHost(fe->rds_count); }
     delete fe;
 }
 
@@ -375,7 +445,8 @@ static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
     case B200_DEMOD_RAW: break;
     case B200_DEMOD_WFM: rc = v->chain.add_wfm(c.deviation, c.out_samplerate, c.low_pass != 0, false); break;
     case B200_DEMOD_WFM_STEREO: rc = v->chain.add_wfm(c.deviation, c.out_samplerate, c.low_pass != 0, true); break;
-    case B200_DEMOD_WFM_RDS: rc = v->chain.add_wfm_rds(c.deviation, c.out_samplerate); break;
+    case B200_DEMOD_WFM_RDS:
+    case B200_DEMOD_WFM_RDS_BITS: rc = v->chain.add_wfm_rds(c.deviation, c.out_samplerate); break;
     case B200_DEMOD_NFM: rc = v->chain.add_nfm(c.out_samplerate, c.bandwidth, c.low_pass != 0); break;
     case B200_DEMOD_AM: rc = v->chain.add_am(c.agc_mode, c.bandwidth, c.agc_attack, c.agc_decay, c.dc_block_rate, c.out_samplerate); break;
     case B200_DEMOD_USB: rc = v->chain.add_ssb(0, c.bandwidth, c.out_samplerate, c.agc_attack, c.agc_decay); break;
@@ -384,7 +455,7 @@ static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
     default: set_error("unknown demodulator %d", c.demod); return B200_EINVAL;
     }
     if (rc) { return rc; }
-    const bool audio = c.demod != B200_DEMOD_RAW && c.demod != B200_DEMOD_WFM_RDS;     // the AF chain and the volume follow audio only
+    const bool audio = c.demod != B200_DEMOD_RAW && c.demod != B200_DEMOD_WFM_RDS && c.demod != B200_DEMOD_WFM_RDS_BITS;     // the AF chain and the volume follow audio only
     if (c.af_samplerate > 0 && audio) {
         if ((rc = v->chain.add_af_chain(c.out_samplerate, c.af_samplerate, c.af_high_pass != 0, c.af_deemph_tau))) { return rc; }
     }
@@ -396,7 +467,23 @@ static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
         // overlapped mode hands every chain's output to the tail stream: give a stage-1-only chain an exact copy stage
         if ((rc = v->chain.add_fir_c(std::vector<float>{ 1.0f }, 1))) { return rc; }
     }
-    return v->chain.finalize(fe->max_eff, ov, &fe->sch.fuse);
+    if ((rc = v->chain.finalize(fe->max_eff, ov, &fe->sch.fuse))) { return rc; }
+    if (c.demod == B200_DEMOD_WFM_RDS_BITS) {
+        if (!fe->rds_count && cudaMallocHost((void**)&fe->rds_count, sizeof(int) * FE_SLOTS * B200_MAX_VFOS) != cudaSuccess) {
+            fe->rds_count = nullptr;
+            return cuda_fail(cudaGetLastError(), "cudaMallocHost");
+        }
+        v->rds = std::make_unique<RdsCore>();
+        if ((rc = v->rds->create(nullptr))) { return rc; }
+        return v->rds_rec.alloc((size_t)b200_rds_demod_max_out(v->chain.max_out(fe->max_eff)) * sizeof(RdsSym), false);
+    }
+    return 0;
+}
+
+// what one chunk of `count` samples can put into a VFO's output buffer, in 8-byte elements
+static int vfo_out_bound(const VfoSlot* v, int count) {
+    const int n = v->chain.max_out(count);
+    return v->rds ? b200_rds_demod_max_out(n) : n;
 }
 
 extern "C" int b200_fe_add_vfo(b200_fe* fe, const b200_vfo_cfg* cfg) {
@@ -464,7 +551,7 @@ extern "C" int b200_fe_vfo_count(b200_fe* fe) {
 extern "C" int b200_fe_vfo_max_out(b200_fe* fe, int id, int count) {
     VfoSlot* v = get_vfo(fe, id);
     if (!v) { return B200_EINVAL; }
-    return v->chain.max_out(count);
+    return vfo_out_bound(v, count);
 }
 extern "C" int b200_fe_fft_max_lines(b200_fe* fe, int count) {
     if (!fe || !fe->fft_on) { return 0; }
@@ -550,6 +637,7 @@ extern "C" int b200_fe_reset(b200_fe* fe) {
     B200_CK(cudaDeviceSynchronize());
     for (auto& v : fe->vfos) {
         if (v->used) { v->chain.reset_state(); }
+        if (v->used && v->rds) { int rcr = v->rds->reset(nullptr); if (rcr) { return rcr; } }
     }
     int rc = fe->sch.reset_raw();
     if (!fe->pre.st.empty()) { fe->pre.reset_state(); }
@@ -708,7 +796,7 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
     const int ecount = (fe->decim > 1) ? fe->pre.peek(count) : count;
     if (ecount < 0) { set_error("input decimator is not a FIR cascade"); return B200_ESTATE; }
     for (size_t k = 0; k < chains.size(); k++) {
-        int bound = chains[k]->max_out(ecount);
+        int bound = vfo_out_bound(fe->vfos[ids[k]].get(), ecount);
         if (out->vfo_out[ids[k]] == nullptr || out->vfo_cap[ids[k]] < bound) {
             set_error("VFO %d output buffer too small: need room for %d samples (b200_fe_vfo_max_out)", ids[k], bound);
             return B200_ECAP;
@@ -798,7 +886,8 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
     std::vector<char> vdirect(chains.size(), direct ? 1 : 0);
     for (size_t k = 0; k < chains.size(); k++) {
         if (host_direct && host_buffer_is_ours(out->vfo_out[ids[k]], (size_t)out->vfo_cap[ids[k]] * chains[k]->out_es * sizeof(float))) { vdirect[k] = 1; }
-        chains[k]->out_override = vdirect[k] ? (float*)out->vfo_out[ids[k]] : nullptr;
+        // an RDS VFO's chain output stays in the chain: RDSDemod reads it there and writes the caller's buffer itself
+        chains[k]->out_override = (vdirect[k] && !fe->vfos[ids[k]]->rds) ? (float*)out->vfo_out[ids[k]] : nullptr;
     }
     fe->lines_override = direct ? out->fft_out : nullptr;
     int nlines = 0;
@@ -812,6 +901,32 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
     // host-side outputs leave through per-VFO device buffers that the copies of the previous chunk may still be reading
     if (!direct && fe->nsub > 0) { B200_CK(cudaStreamWaitEvent(fe->sch.out_stream(), fe->ev_out[(slot + FE_SLOTS - 1) % FE_SLOTS], 0)); }
     if ((rc = fe->sch.run(chains, dptr, in_fmt, count, true))) { return rc; }
+    // RDSDemod behind the WFM_RDS_BITS VFOs: one launch per B200_BATCH of those with 5 kS/s samples this chunk, on the stream of
+    // the tails, behind them and in front of the next chunk's (which overwrite the chain outputs and move the RDS states)
+    fe->rds_pend[slot].clear();
+    fe->rds_out[slot] = out;
+    if (fe->rds_count) {         // allocated with the first WFM_RDS_BITS VFO: a handle that never had one skips all this
+        RdsParams rp;
+        memset(&rp, 0, sizeof(rp));
+        auto flush = [&]() -> int {
+            cudaError_t e = launch_rds_demod(rp, fe->sch.out_stream());
+            if (e != cudaSuccess) { return cuda_fail(e, "launch_rds_demod"); }
+            fe->sch.launches += rp.njobs > 0 ? 1 : 0;
+            rp.njobs = 0;
+            return 0;
+        };
+        for (size_t k = 0; k < chains.size(); k++) {
+            VfoSlot* v = fe->vfos[ids[k]].get();
+            if (!v->rds) { continue; }
+            const int n = chains[k]->n_out, bound = b200_rds_demod_max_out(n);
+            fe->rds_pend[slot].push_back({ ids[k], n, bound });
+            if (n == 0) { continue; }
+            RdsSym* dst = vdirect[k] ? (RdsSym*)out->vfo_out[ids[k]] : v->rds_rec.as<RdsSym>();
+            rp.job[rp.njobs++] = v->rds->job(chains[k]->out.as<float2>(), n, dst, bound, fe->rds_count + slot * B200_MAX_VFOS + ids[k]);
+            if (rp.njobs == B200_BATCH && (rc = flush())) { return rc; }
+        }
+        if ((rc = flush())) { return rc; }
+    }
     const long long hp3 = host_clock_ns();
     // join on a stream of its own: the VFO branch (tail stream) and the spectrum branch (its stream) of this chunk meet
     // here, neither waits for the other -- the tail stream goes straight on to the next chunk
@@ -830,6 +945,14 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
     const cudaMemcpyKind kind = (out->out_mem == B200_MEM_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     for (size_t k = 0; k < chains.size(); k++) {
         Chain* c = chains[k];
+        if (fe->vfos[ids[k]]->rds) {
+            // the symbol count is known after the launch: every record the bound allows leaves, b200_fe_wait sets the count
+            const int bound = b200_rds_demod_max_out(c->n_out);
+            if (c->n_out > 0 && !vdirect[k]) {
+                B200_CK(cudaMemcpyAsync(out->vfo_out[ids[k]], fe->vfos[ids[k]]->rds_rec.p, (size_t)bound * sizeof(RdsSym), kind, os));
+            }
+            continue;
+        }
         out->vfo_count[ids[k]] = c->n_out;
         if (c->n_out > 0 && !vdirect[k]) {
             B200_CK(cudaMemcpyAsync(out->vfo_out[ids[k]], c->out.p, (size_t)c->n_out * c->out_es * sizeof(float), kind, os));
@@ -856,7 +979,18 @@ extern "C" int b200_fe_wait(b200_fe* fe) {
     B200_CK(cudaEventSynchronize(fe->ev_out[slot]));
     fe->nwait++;
     if (trace_on() && fe->nwait == fe->nsub && fe->nsub >= 8) { trace_dump("chunks in flight drained"); }
-    return 0;
+    int rc = 0;
+    for (const auto& p : fe->rds_pend[slot]) {
+        const int n = p.n_in > 0 ? fe->rds_count[slot * B200_MAX_VFOS + p.id] : 0;
+        if (n < 0 || n > p.bound) {
+            set_error("VFO %d: RDS clock recovery produced %d symbols from %d samples (bound %d)", p.id, n, p.n_in, p.bound);
+            rc = B200_ECAP;
+            continue;
+        }
+        fe->rds_out[slot]->vfo_count[p.id] = n;
+    }
+    fe->rds_pend[slot].clear();
+    return rc;
 }
 
 extern "C" int b200_fe_process(b200_fe* fe, const void* iq, int count, int in_fmt, int in_mem, b200_outputs* out) {
@@ -1160,19 +1294,17 @@ extern "C" int b200_block_reset(b200_block* b) {
     return b->sch.reset_raw();
 }
 
-// ------------------------------------------------------------------ RDSDemod (decoder_modules/radio/src/rds_demod.h)
-// Not a Chain stage: the clock recovery's output count depends on the data, so it cannot be mirrored on the host like the
-// counts of every other block; the count comes back with the symbols (one small copy + one synchronisation per call at 5 kS/s).
+// ------------------------------------------------------------------ RDSDemod as a stand-alone block (RdsCore above)
+// The clock recovery's output count depends on the data: it comes back with the symbols (one small copy + one synchronisation
+// per call at 5 kS/s).  A front-end VFO in B200_DEMOD_WFM_RDS_BITS mode runs the same kernel without that synchronisation.
 struct b200_rds_demod {
     cudaStream_t stream = nullptr;
-    DevBuf in, soft, hard, state, taps, bank;
-    RdsState init;               // what reset() restores
-    RdsJob proto;
+    RdsCore core;
+    DevBuf in, rec;
     int max_chunk = 1000000;     // STREAM_BUFFER_SIZE (core/src/dsp/stream.h:9)
     int out_cap = 0;
-    RdsState* hstate = nullptr;  // pinned: the state block (with the symbol count) after a launch
-    float* hsoft = nullptr;      // pinned staging of the symbols
-    unsigned char* hhard = nullptr;
+    RdsSym* hrec = nullptr;      // pinned staging of the symbols
+    int* hcount = nullptr;       // pinned: the symbol count of the last launch, written by the kernel
     long long launches = 0;
     std::mutex mtx;              // process() and reset() may come from different threads (worker / control), like the other blocks
 };
@@ -1185,9 +1317,8 @@ extern "C" int b200_rds_demod_max_out(int count) {
 extern "C" void b200_rds_demod_destroy(b200_rds_demod* r) {
     if (!r) { return; }
     if (r->stream) { cudaStreamSynchronize(r->stream); cudaStreamDestroy(r->stream); }
-    if (r->hstate) { cudaFreeHost(r->hstate); }
-    if (r->hsoft) { cudaFreeHost(r->hsoft); }
-    if (r->hhard) { cudaFreeHost(r->hhard); }
+    if (r->hrec) { cudaFreeHost(r->hrec); }
+    if (r->hcount) { cudaFreeHost(r->hcount); }
     delete r;
 }
 extern "C" b200_rds_demod* b200_rds_demod_create(void) {
@@ -1195,43 +1326,13 @@ extern "C" b200_rds_demod* b200_rds_demod_create(void) {
     b200_rds_demod* r = new b200_rds_demod;
     int rc = 0;
     if (cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "cudaStreamCreate"); r->stream = nullptr; }
-    // init() of rds_demod.h:20-41
-    const std::vector<float> bp = bandpass_c_taps(0.0, 2375.0, 100.0, 5000.0, false);      // (re, im) pairs
-    const std::vector<float> bank = mm_interp_bank(RDS_MM_PHASES, RDS_MM_TAPS);
-    const int nt = (int)bp.size() / 2;
-    if (!rc && (nt < 2 || nt > RDS_MAXTAPS)) { set_error("RDS band-pass of %d taps", nt); rc = B200_EINVAL; }
     r->out_cap = b200_rds_demod_max_out(r->max_chunk);
     if (!rc) { rc = r->in.alloc((size_t)r->max_chunk * sizeof(float2), false); }
-    if (!rc) { rc = r->soft.alloc((size_t)r->out_cap * sizeof(float), false); }
-    if (!rc) { rc = r->hard.alloc((size_t)r->out_cap, false); }
-    if (!rc) { rc = r->state.alloc(sizeof(RdsState), false); }
-    if (!rc) { rc = r->taps.alloc(bp.size() * sizeof(float), false); }
-    if (!rc) { rc = r->bank.alloc(bank.size() * sizeof(float), false); }
-    if (!rc && cudaMallocHost((void**)&r->hstate, sizeof(RdsState)) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "cudaMallocHost"); }
-    if (!rc && cudaMallocHost((void**)&r->hsoft, (size_t)r->out_cap * sizeof(float)) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "cudaMallocHost"); }
-    if (!rc && cudaMallocHost((void**)&r->hhard, (size_t)r->out_cap) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "cudaMallocHost"); }
+    if (!rc) { rc = r->rec.alloc((size_t)r->out_cap * sizeof(RdsSym), false); }
+    if (!rc && cudaMallocHost((void**)&r->hrec, (size_t)r->out_cap * sizeof(RdsSym)) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "cudaMallocHost"); }
+    if (!rc && cudaMallocHost((void**)&r->hcount, sizeof(int)) != cudaSuccess) { rc = cuda_fail(cudaGetLastError(), "cudaMallocHost"); }
+    if (!rc) { rc = r->core.create(r->stream); }
     if (rc) { b200_rds_demod_destroy(r); return nullptr; }
-    RdsJob& J = r->proto;
-    memset(&J, 0, sizeof(J));
-    J.ntaps = nt;
-    J.set_point = (float)1.0; J.max_gain = (float)1e6; J.rate = (float)0.1;               // agc.init(NULL, 1.0, 1e6, 0.1)
-    pll_coefficients(0.005f, J.c1_alpha, J.c1_beta);                                       // costas.init(NULL, 0.005f)
-    J.c1_min = -3.1415926535f; J.c1_max = 3.1415926535f;                                   // FL_M_PI (math/constants.h:4)
-    const double baud = hz_to_rads(2375.0 / 2.0, 5000.0);
-    pll_coefficients(0.01, J.c2_alpha, J.c2_beta);                                         // costas2.init(NULL, 0.01, 0, f, f - 10 %, f + 10 %)
-    J.c2_min = (float)(baud - (baud * 0.1)); J.c2_max = (float)(baud + (baud * 0.1));
-    const double omega = 5000.0 / (2375.0 / 2.0);                                          // recov.init(NULL, omega, 1e-6, 0.01, 0.01)
-    J.mm_alpha = (float)0.01; J.mm_beta = (float)1e-6;
-    J.mm_min = (float)(omega * (1.0 - 0.01)); J.mm_max = (float)(omega * (1.0 + 0.01));
-    memset(&r->init, 0, sizeof(r->init));
-    r->init.gain = (float)1.0;
-    r->init.c2_freq = (float)baud;
-    r->init.mm_freq = (float)omega;
-    cudaError_t e = cudaMemcpyAsync(r->taps.p, bp.data(), bp.size() * sizeof(float), cudaMemcpyHostToDevice, r->stream);
-    if (e == cudaSuccess) { e = cudaMemcpyAsync(r->bank.p, bank.data(), bank.size() * sizeof(float), cudaMemcpyHostToDevice, r->stream); }
-    if (e == cudaSuccess) { e = cudaMemcpyAsync(r->state.p, &r->init, sizeof(RdsState), cudaMemcpyHostToDevice, r->stream); }
-    if (e == cudaSuccess) { e = cudaStreamSynchronize(r->stream); }
-    if (e != cudaSuccess) { cuda_fail(e, "RDS demodulator tables"); b200_rds_demod_destroy(r); return nullptr; }
     return r;
 }
 extern "C" int b200_rds_demod_process(b200_rds_demod* r, int count, const void* in, float* soft, uint8_t* hard) {
@@ -1243,40 +1344,27 @@ extern "C" int b200_rds_demod_process(b200_rds_demod* r, int count, const void* 
     B200_CK(cudaMemcpyAsync(r->in.p, in, (size_t)count * sizeof(float2), cudaMemcpyDefault, s));      // host or device memory
     RdsParams p;
     memset(&p, 0, sizeof(p));
-    p.njobs = 1;
-    p.job[0] = r->proto;
-    RdsJob& J = p.job[0];
-    J.in = r->in.as<float2>(); J.soft = r->soft.as<float>(); J.hard = r->hard.as<unsigned char>();
-    J.state = r->state.as<RdsState>(); J.taps = r->taps.as<float2>(); J.bank = r->bank.as<float>();
     const int bound = std::min(r->out_cap, b200_rds_demod_max_out(count));
-    J.n = count; J.out_cap = bound;
+    p.njobs = 1;
+    p.job[0] = r->core.job(r->in.as<float2>(), count, r->rec.as<RdsSym>(), bound, r->hcount);
     cudaError_t e = launch_rds_demod(p, s);
     if (e != cudaSuccess) { return cuda_fail(e, "launch_rds_demod"); }
     r->launches++;
-    B200_CK(cudaMemcpyAsync(r->hstate, r->state.p, sizeof(RdsState), cudaMemcpyDeviceToHost, s));
-    B200_CK(cudaMemcpyAsync(r->hsoft, r->soft.p, (size_t)bound * sizeof(float), cudaMemcpyDeviceToHost, s));
-    B200_CK(cudaMemcpyAsync(r->hhard, r->hard.p, (size_t)bound, cudaMemcpyDeviceToHost, s));
+    B200_CK(cudaMemcpyAsync(r->hrec, r->rec.p, (size_t)bound * sizeof(RdsSym), cudaMemcpyDeviceToHost, s));
     B200_CK(cudaStreamSynchronize(s));
-    const int n = r->hstate->out_count;
+    const int n = *r->hcount;
     if (n < 0 || n > bound) { set_error("RDS clock recovery produced %d symbols from %d samples (bound %d)", n, count, bound); return B200_ECAP; }
-    memcpy(soft, r->hsoft, (size_t)n * sizeof(float));
-    memcpy(hard, r->hhard, (size_t)n);
+    for (int i = 0; i < n; i++) {
+        soft[i] = r->hrec[i].soft;
+        hard[i] = (uint8_t)r->hrec[i].bit;
+    }
     return n;
 }
 extern "C" int b200_rds_demod_reset(b200_rds_demod* r) {
     if (!r) { set_error("null block"); return B200_EINVAL; }
-    // RDSDemod::reset (rds_demod.h:52-62): gain, loop phases / frequencies, band-pass delay line, MM offset / phase / lastOut,
-    // decoder memory.  MM::reset (mm.h:83-92) leaves its work-buffer tail alone: so does this.
     std::lock_guard<std::mutex> lk(r->mtx);
     B200_CK(cudaStreamSynchronize(r->stream));
-    B200_CK(cudaMemcpyAsync(r->hstate, r->state.p, sizeof(RdsState), cudaMemcpyDeviceToHost, r->stream));
-    B200_CK(cudaStreamSynchronize(r->stream));
-    RdsState st = r->init;
-    memcpy(st.m_hist, r->hstate->m_hist, sizeof(st.m_hist));
-    *r->hstate = st;
-    B200_CK(cudaMemcpyAsync(r->state.p, r->hstate, sizeof(RdsState), cudaMemcpyHostToDevice, r->stream));
-    B200_CK(cudaStreamSynchronize(r->stream));
-    return 0;
+    return r->core.reset(r->stream);
 }
 extern "C" long long b200_rds_demod_launch_count(b200_rds_demod* r) { return r ? r->launches : 0; }
 /* test hooks: the two tap sets of the block as the host designs them */

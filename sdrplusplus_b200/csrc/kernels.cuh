@@ -264,15 +264,15 @@ struct RdsState {
     float c2_phase, c2_freq;            // second Costas loop
     float mm_phase, mm_freq, last_out;  // MM: pcl.phase (mu), pcl.freq (omega), lastOut
     int offset, diff_last;              // MM::offset, DifferentialDecoder::last
-    int out_count;                      // symbols of the last launch
-    int pad;
     float2 c1_hist[RDS_MAXTAPS];        // band-pass delay line (ntaps - 1 used)
     float m_hist[RDS_MM_TAPS];          // MM work-buffer tail (7 used)
 };
+// one recovered symbol: RDSDemod::soft and the differentially decoded bit of RDSDemod::out (b200_rds_symbol of b200dsp.h)
+struct RdsSym { float soft; unsigned int bit; };
 struct RdsJob {
     const float2* in;       // n complex samples at 5 kS/s
-    float* soft;            // out_cap
-    unsigned char* hard;    // out_cap
+    RdsSym* out;            // out_cap records (device memory or mapped pinned host memory)
+    int* count;             // symbols of this launch (out_cap + 1 when the capacity ran out); its own slot per launch
     RdsState* state;
     const float2* taps;     // band-pass, complex
     const float* bank;      // [RDS_MM_PHASES][RDS_MM_TAPS]

@@ -15,6 +15,8 @@
 // contraction: which interpolator phase and which sample the clock recovery picks are decisions of the fed-back value); all
 // threads run the band-pass, two interleaved partial sums like the generic complex dot product of the oracle's leaf layer.
 // 5 kS/s per stream: this is not a throughput kernel (a 16 Mi-sample chunk of a 100 MS/s stream carries 839 samples of it).
+// Callers: the stand-alone b200_rds_demod (one job per call) and the front end's B200_DEMOD_WFM_RDS_BITS VFOs (up to B200_BATCH
+// jobs per launch).  Each job writes b200_rds_symbol records and its symbol count to a count slot of its own.
 #pragma once
 
 #define RDS_TILE 1024
@@ -119,8 +121,7 @@ __global__ void __launch_bounds__(RDS_THREADS) k_rds_demod(const __grid_constant
                 for (int k = 0; k < RDS_MM_TAPS; k++) { acc = __fadd_rn(acc, __fmul_rn(mb[offset + k], bank[ph * RDS_MM_TAPS + k])); }
                 const int bit = acc > 0.0f ? 1 : 0;
                 if (nout < J.out_cap) {
-                    J.soft[nout] = acc;
-                    J.hard[nout] = (unsigned char)((bit - dlast + 2) % 2);                  // slicer + differential decoder
+                    J.out[nout] = RdsSym{ acc, (unsigned int)((bit - dlast + 2) % 2) };    // slicer + differential decoder
                 }
                 dlast = bit;
                 nout++;
@@ -160,7 +161,7 @@ __global__ void __launch_bounds__(RDS_THREADS) k_rds_demod(const __grid_constant
     if (tid == 0) {
         S->gain = gain; S->c1_phase = p1; S->c1_freq = f1; S->c2_phase = p2; S->c2_freq = f2;
         S->mm_phase = mph; S->mm_freq = mfr; S->last_out = last; S->offset = offset; S->diff_last = dlast;
-        S->out_count = nout;
+        *J.count = nout;
     }
 }
 

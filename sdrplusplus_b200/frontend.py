@@ -73,6 +73,11 @@ class VfoConfig:
         return VfoConfig(offset, 250000.0, bandwidth, L.DEMOD_WFM_RDS, deviation=bandwidth / 2.0)
 
     @staticmethod
+    def wfm_rds_bits(offset, bandwidth=150000.0):
+        # the same branch followed by RDSDemod: one (soft, bit) record per recovered symbol
+        return VfoConfig(offset, 250000.0, bandwidth, L.DEMOD_WFM_RDS_BITS, deviation=bandwidth / 2.0)
+
+    @staticmethod
     def nfm(offset, bandwidth=12500.0):
         return VfoConfig(offset, 50000.0, bandwidth, L.DEMOD_NFM, low_pass=True)          # nfm.h:29,56-58
 
@@ -100,6 +105,13 @@ class VfoConfig:
 
 
 _NP_FMT = {L.FMT_CF32: (np.complex64, 1), L.FMT_CS16: (np.int16, 2), L.FMT_CS8: (np.int8, 2)}
+RDS_SYMBOL = np.dtype([("soft", np.float32), ("bit", np.uint32)])      # b200_rds_symbol
+
+
+def rds_symbols(buf, n):
+    """(soft float32, bit uint8) of the first n b200_rds_symbol records in a float32 output buffer"""
+    r = np.ascontiguousarray(buf[: 2 * n]).view(RDS_SYMBOL)
+    return r["soft"].copy(), r["bit"].astype(np.uint8)
 
 
 def _as_input(iq, fmt):
@@ -218,13 +230,17 @@ class FrontEnd:
         return o, bufs, fft
 
     def process(self, iq, fmt=L.FMT_CF32):
-        """Host numpy in, host numpy out.  Returns ({vfo_id: array}, fft_lines[n, N])."""
+        """Host numpy in, host numpy out.  Returns ({vfo_id: array}, fft_lines[n, N]); a DEMOD_WFM_RDS_BITS VFO gives the
+        pair (soft float32, bit uint8)."""
         a, count = _as_input(iq, fmt)
         o, bufs, fft = self._alloc_outputs(count)
         L.check(self._l.b200_fe_process(self._h, a.ctypes.data, count, fmt, L.MEM_HOST, C.byref(o)))
         outs = {}
         for vid, cfg in self.vfos.items():
             n = o.vfo_count[vid]
+            if cfg.demod == L.DEMOD_WFM_RDS_BITS:
+                outs[vid] = rds_symbols(bufs[vid], n)
+                continue
             y = bufs[vid][: 2 * n].copy()
             outs[vid] = y.view(np.complex64) if cfg.demod in (L.DEMOD_RAW, L.DEMOD_WFM_RDS) else y.reshape(-1, 2)
         lines = fft[: o.fft_lines].copy() if fft is not None else np.empty((0, 0), np.float32)
@@ -241,7 +257,13 @@ class FrontEnd:
                 acc[vid].append(y)
             if ln.size:
                 lines.append(ln)
-        res = {vid: (np.concatenate(v) if v else np.empty(0, np.float32)) for vid, v in acc.items()}
+        res = {}
+        for vid, v in acc.items():
+            if self.vfos[vid].demod == L.DEMOD_WFM_RDS_BITS:
+                res[vid] = (np.concatenate([p[0] for p in v]) if v else np.empty(0, np.float32),
+                            np.concatenate([p[1] for p in v]) if v else np.empty(0, np.uint8))
+            else:
+                res[vid] = np.concatenate(v) if v else np.empty(0, np.float32)
         return res, (np.concatenate(lines) if lines else np.empty((0, self.fft_size), np.float32))
 
     # raw-pointer variants used by bench.py (device-resident or pinned buffers, no numpy copies)

@@ -66,7 +66,10 @@ namespace dsp::b200 {
         void setFFTSize(int fftSize) { size = fftSize; updateFFTPath(); }
         void setFFTRate(double rate) { _rate = rate; updateFFTPath(); }
         void setFFTWindow(int window) { _window = window; updateFFTPath(); }
+        // every VFO's output stream has 8-byte elements: stereo_t audio, complex_t for B200_DEMOD_RAW / B200_DEMOD_WFM_RDS, and
+        // one b200_rds_symbol per recovered symbol for B200_DEMOD_WFM_RDS_BITS (read them with rdsSymbols)
         stream<stereo_t>* vfoOut(int id) { return outs_[id]; }
+        static const b200_rds_symbol* rdsSymbols(const stream<stereo_t>* s) { return (const b200_rds_symbol*)s->readBuf; }
 
         int run() override {
             int count = _in->read();

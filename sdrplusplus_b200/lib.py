@@ -12,6 +12,7 @@ FMT_CF32, FMT_CS16, FMT_CS8 = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
 WIN_RECTANGULAR, WIN_BLACKMAN, WIN_NUTTALL = 0, 1, 2
 DEMOD_RAW, DEMOD_WFM, DEMOD_NFM, DEMOD_AM, DEMOD_USB, DEMOD_LSB, DEMOD_DSB, DEMOD_WFM_STEREO, DEMOD_WFM_RDS = range(9)
+DEMOD_WFM_RDS_BITS = 9
 AGC_CARRIER, AGC_AUDIO = 0, 1
 E = {0: "OK", -1: "EINVAL", -2: "ENODEV", -3: "ECUDA", -4: "ENOMEM", -5: "ECAP", -6: "ENOPLAN", -7: "ESTATE"}
 
@@ -34,6 +35,11 @@ class VfoCfg(C.Structure):
 class Outputs(C.Structure):
     _fields_ = [("vfo_out", C.c_void_p * MAX_VFOS), ("vfo_cap", C.c_int * MAX_VFOS), ("vfo_count", C.c_int * MAX_VFOS),
                 ("fft_out", C.c_void_p), ("fft_cap_lines", C.c_int), ("fft_lines", C.c_int), ("out_mem", C.c_int)]
+
+
+class RdsSymbol(C.Structure):
+    """b200_rds_symbol: one record per recovered symbol of a DEMOD_WFM_RDS_BITS VFO"""
+    _fields_ = [("soft", C.c_float), ("bit", C.c_uint32)]
 
 
 class ResampPlan(C.Structure):
