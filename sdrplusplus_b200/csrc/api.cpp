@@ -109,7 +109,7 @@ static int ilog2(int n) { int l = 0; while ((1 << l) < n) { l++; } return l; }
 
 struct FftCore {
     FftPlanDev plan;
-    DevBuf tw, twf, win, work;
+    DevBuf tw, twf, win, winp, work;
     int size = 0, nz = 0, window = 0;
     int create(int size_, int nz_, int window_, int max_batch = 1) {
         if (size_ < 8 || size_ > (1 << 22) || (size_ & (size_ - 1))) { set_error("FFT size %d must be a power of two in [8, 4194304]", size_); return B200_EINVAL; }
@@ -148,6 +148,24 @@ struct FftCore {
             if ((rc = twf.alloc(f.size() * sizeof(float2)))) { return rc; }
             B200_CK(cudaMemcpy(twf.p, f.data(), f.size() * sizeof(float2), cudaMemcpyHostToDevice));
             plan.tw_fine = twf.as<float2>();
+        }
+        plan.window_p = nullptr;
+        if (fft_plan_uses_reg(plan)) {
+            // pass 1 of the register FFT: thread t of column n2 multiplies x[(a RB + t) N2 + n2], a < RA, by the window.
+            // Laid out as winp[(n2 RB + t) RA + a], those RA values are one contiguous run the thread reads in 16-byte vectors.
+            const int RA = plan.logN1 == 8 ? 16 : (plan.logN1 == 9 ? 16 : 32), RB = plan.logN1 == 8 ? 16 : 32;
+            std::vector<float> wp((size_t)size, 0.0f);
+            for (int n2 = 0; n2 < plan.N2; n2++) {
+                for (int t = 0; t < RB; t++) {
+                    for (int a = 0; a < RA; a++) {
+                        const long long n = (long long)(a * RB + t) * plan.N2 + n2;
+                        if (n < nz) { wp[((size_t)n2 * RB + t) * RA + a] = w[(size_t)n]; }
+                    }
+                }
+            }
+            if ((rc = winp.alloc(wp.size() * sizeof(float)))) { return rc; }
+            B200_CK(cudaMemcpy(winp.p, wp.data(), wp.size() * sizeof(float), cudaMemcpyHostToDevice));
+            plan.window_p = winp.as<float>();
         }
         B200_CK(cudaDeviceSynchronize());       // tables uploaded on the legacy stream; the spectrum branch runs on a non-blocking one
         return 0;
@@ -253,6 +271,14 @@ struct b200_fe {
     DevBuf frame, lines;
     int max_lines = 0;
     unsigned long long pos = 0, fstart = 0;
+    // frame[0 .. pos - fstart) holds the part of the frame at fstart that earlier chunks carried, in format frame_fmt at
+    // ingest scale frame_scale (cf32: already scaled)
+    int frame_fmt = FMT_CF32;
+    float frame_scale = 0.0f;
+    // 1: a frame that began in earlier chunks joins its chunk's batch, staged by copies in the input's format; the register
+    // passes read their twiddles from shared memory.  0: the frame is converted to cf32 and transformed on its own, twiddles
+    // from global memory.  Same lines either way.
+    int fft_v = 1;
     // pipelining
     cudaEvent_t ev_h2d[FE_SLOTS] = {}, ev_compute[FE_SLOTS] = {}, ev_out[FE_SLOTS] = {};
     bool slot_used[FE_SLOTS] = {};
@@ -613,6 +639,12 @@ extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {
         return 0;
     }
     if (!strcmp(key, "fft_serial")) { fe->fft_serial = value; return 0; }
+    if (!strcmp(key, "fft_v")) {
+        if (value != 0 && value != 1) { set_error("fft_v: 0 or 1"); return B200_EINVAL; }
+        std::lock_guard<std::mutex> lck(fe->mtx);
+        fe->fft_v = value;
+        return 0;
+    }
     if (!strcmp(key, "graph")) { fe->sch.graph_tails = value; if (value == 0) { fe->sch.drop_graphs(); } return 0; }
     if (!strcmp(key, "graph_max_count")) { fe->sch.graph_max_count = value; return 0; }
     if (!strcmp(key, "pdl")) { kernels_set_pdl(value); fe->sch.drop_graphs(); return 0; }      // process-wide, like the kernel variants
@@ -716,8 +748,23 @@ static int fe_fft_chunk(b200_fe* fe, const void* dptr, int fmt, int count, int* 
         return 0;
     };
     int rc = 0;
-    // 1) a frame that started in an earlier chunk: stage this chunk's part, transform it if it completes here
-    if (fe->fstart < pos) {
+    char* const frame = (char*)fe->frame.p;
+    // a frame begun in earlier chunks whose staged part this chunk cannot extend in place (other format or scale, or the
+    // cf32 staging of fft_v 0): convert that part to cf32 through the work buffer, and carry the frame on in cf32
+    const bool pending = fe->fstart < pos;
+    const bool same_fmt = fe->frame_fmt == fmt && (fmt == FMT_CF32 || fe->frame_scale == isc);
+    if (pending && (!fe->fft_v || !same_fmt) && fe->frame_fmt != FMT_CF32) {
+        if ((rc = fork())) { return rc; }
+        const int len = (int)(pos - fe->fstart);
+        cudaError_t e = launch_convert_cf32(frame, fe->frame_fmt, fe->fft.work.as<float2>(), len, fe->frame_scale, s);
+        if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
+        fe->sch.launches++;
+        B200_CK(cudaMemcpyAsync(frame, fe->fft.work.p, (size_t)len * sizeof(float2), cudaMemcpyDeviceToDevice, s));
+        fe->frame_fmt = FMT_CF32;
+        fe->frame_scale = 0.0f;
+    }
+    if (pending && (!fe->fft_v || !same_fmt)) {
+        // 1) this chunk's part of the frame, converted behind the staged cf32 part; transformed alone if it completes here
         const unsigned long long fend = fe->fstart + nz;
         const unsigned long long lo = pos, hi = std::min(fend, end);
         if (hi > lo) {
@@ -729,23 +776,32 @@ static int fe_fft_chunk(b200_fe* fe, const void* dptr, int fmt, int count, int* 
         if (fend <= end) {
             if ((rc = fork())) { return rc; }
             int nl = 0;
-            cudaError_t e = launch_fft_frame(fe->fft.plan, fe->frame.p, FMT_CF32, fe->fft.work.as<float2>(), lines_base, nullptr, s, &nl);
-            if (e != cudaSuccess) { return cuda_fail(e, "launch_fft_frame"); }
+            const FftFrames fr{ fe->frame.p, nullptr, 0, 0, 1 };
+            cudaError_t e = launch_fft_frames(fe->fft.plan, fr, FMT_CF32, fe->fft.work.as<float2>(), lines_base, nullptr, s, &nl, fe->fft_v != 0);
+            if (e != cudaSuccess) { return cuda_fail(e, "launch_fft_frames"); }
             fe->sch.launches += nl;
             (*nlines)++;
             fe->fstart += interval;
         }
     }
-    // 2) frames that lie completely inside this chunk: one batched launch pair, read straight from the chunk
-    if (fe->fstart >= pos && fe->fstart + nz <= end) {
+    else if (pending && fe->fstart + nz > end) {
+        // a frame that spans this whole chunk: append the chunk to its staged part
+        if (count > 0) {
+            if ((rc = fork())) { return rc; }
+            B200_CK(cudaMemcpyAsync(frame + (size_t)(pos - fe->fstart) * bps, dptr, (size_t)count * bps, cudaMemcpyDeviceToDevice, s));
+        }
+    }
+    // 2) the frames that complete in this chunk, one batched launch pair.  With fft_v 1 the first may have begun in earlier
+    // chunks: its first `split` samples come from the staged part, the rest straight from the chunk.
+    const unsigned long long split = fe->fstart < pos ? pos - fe->fstart : 0;
+    if (fe->fstart + nz <= end) {
         int nb = (int)((end - fe->fstart - nz) / interval) + 1;
         if (*nlines + nb > fe->max_lines) { set_error("FFT line buffer overflow"); return B200_ECAP; }
         if ((rc = fork())) { return rc; }
-        const char* src = (const char*)dptr + (size_t)(fe->fstart - pos) * bps;
+        const FftFrames fr{ (const char*)dptr + (size_t)(fe->fstart + split - pos) * bps, frame, (long long)interval, (int)split, nb };
         int nl = 0;
-        cudaError_t e = launch_fft_frames(fe->fft.plan, src, fmt, fe->fft.work.as<float2>(),
-                                          lines_base + (size_t)(*nlines) * fe->fft.size, nullptr, s, &nl, nb,
-                                          (long long)interval * bps);
+        cudaError_t e = launch_fft_frames(fe->fft.plan, fr, fmt, fe->fft.work.as<float2>(), lines_base + (size_t)(*nlines) * fe->fft.size,
+                                          nullptr, s, &nl, fe->fft_v != 0);
         if (e != cudaSuccess) { return cuda_fail(e, "launch_fft_frames"); }
         fe->sch.launches += nl;
         *nlines += nb;
@@ -754,12 +810,19 @@ static int fe_fft_chunk(b200_fe* fe, const void* dptr, int fmt, int count, int* 
     // 3) the head of a frame that continues into the next chunk
     if (fe->fstart < end && fe->fstart >= pos) {
         const unsigned long long lo = fe->fstart, hi = end;
-        if (hi > lo) {
-            if ((rc = fork())) { return rc; }
-            const char* src = (const char*)dptr + (size_t)(lo - pos) * bps;
+        if ((rc = fork())) { return rc; }
+        const char* src = (const char*)dptr + (size_t)(lo - pos) * bps;
+        if (fe->fft_v) {
+            B200_CK(cudaMemcpyAsync(frame, src, (size_t)(hi - lo) * bps, cudaMemcpyDeviceToDevice, s));
+            fe->frame_fmt = fmt;
+            fe->frame_scale = isc;
+        }
+        else {
             cudaError_t e = launch_convert_cf32(src, fmt, fe->frame.as<float2>(), (int)(hi - lo), isc, s);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
             fe->sch.launches++;
+            fe->frame_fmt = FMT_CF32;
+            fe->frame_scale = 0.0f;
         }
     }
     if (forked) {

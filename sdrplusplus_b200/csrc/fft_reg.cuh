@@ -59,8 +59,9 @@ template <int RA, int RB> struct FrGeom {
 
 // steps 1 + 2 of one length-n transform.  in: v[a] = x[a*RB + t] (threads t < RB); out: v[d'] with
 // X[t + RA*d] = v[fr_brev<RB>(d)] (threads t < RA).  ex: this transform's exchange tile.
-// twn[m] = exp(-2 pi i m / n) through the plan's table: tw[m << twsh]
-template <int RA, int RB>
+// twn[m] = exp(-2 pi i m / n) through the plan's table: tw[m << twsh], read from global memory (TAB = false) or from the
+// CTA's shared-memory copy of the table (TAB = true)
+template <int RA, int RB, bool TAB>
 __device__ __forceinline__ void fr_transform(float2 (&v)[RA > RB ? RA : RB], float2* ex, int t, const float2* __restrict__ tw, int twsh) {
     using G = FrGeom<RA, RB>;
     if (t < RB) {
@@ -71,7 +72,7 @@ __device__ __forceinline__ void fr_transform(float2 (&v)[RA > RB ? RA : RB], flo
 #pragma unroll
         for (int c = 0; c < RA; c++) {
             float2 y = a[fr_brev<RA>(c)];
-            if (c > 0) { y = cmulf(y, __ldg(tw + ((size_t)(t * c) << twsh))); }
+            if (c > 0) { y = cmulf(y, TAB ? tw[(t * c) << twsh] : __ldg(tw + ((size_t)(t * c) << twsh))); }
             ex[c * G::crow + t] = y;
         }
     }
@@ -86,23 +87,58 @@ __device__ __forceinline__ void fr_transform(float2 (&v)[RA > RB ? RA : RB], flo
     }
 }
 
+// copy n float2 (n even, both 16-byte aligned) from global into shared memory, the whole CTA
+__device__ __forceinline__ void fr_stage_table(float2* dst, const float2* __restrict__ src, int n) {
+    for (int i = threadIdx.x; i < n / 2; i += blockDim.x) {
+        reinterpret_cast<float4*>(dst)[i] = __ldg(reinterpret_cast<const float4*>(src) + i);
+    }
+}
+// shared memory of a register-FFT pass: the exchange tiles of its X transforms, then (TAB) the twiddle tables
+template <int RA, int RB>
+__host__ __device__ constexpr size_t fr_smem_tiles(int X) { return (size_t)X * FrGeom<RA, RB>::pitch; }
+
 // pass 1: CTA = C adjacent columns n2, every row n1:  A[k1][n2] = W_N^(k1 n2) * sum_n1 x[n1 N2 + n2] W_N1^(n1 k1)
-template <int FMT, int RA, int RB, int C, int MINB>
-__global__ void __launch_bounds__(C * FrGeom<RA, RB>::TP, MINB) k_fftr_p1(const __grid_constant__ FftPlanDev pl, const void* __restrict__ src0,
-                                                                    float2* __restrict__ work0, long long src_stride_bytes) {
+// TAB = false: twiddles and window straight from global memory (gathers).  TAB = true: the CTA first copies the coarse
+// and fine twiddle tables (TW + N/TW float2, at most 16 KB) into shared memory -- the same fp32 values, so the same
+// products -- and reads the window from the plan's per-thread layout (window_p) in 16-byte vectors.
+// Registers: at most 144 with the tables (the least at which the 32 x 32 transform does not spill; DESIGN.md section 4 has
+// what then fits on an SM); without them as before: 128 for a CTA of 8 transforms, unbounded for a CTA of 4.
+template <int FMT, int RA, int RB, int C, bool TAB>
+__global__ void __launch_bounds__(C * FrGeom<RA, RB>::TP) __maxnreg__(TAB ? 144 : (C == 8 ? 128 : 255)) k_fftr_p1(const __grid_constant__ FftPlanDev pl, const __grid_constant__ FftFrames fr,
+                                                                    float2* __restrict__ work0) {
     using G = FrGeom<RA, RB>;
     extern __shared__ __align__(16) float2 smem[];
     const int N2 = pl.N2;
-    const void* src = reinterpret_cast<const char*>(src0) + (size_t)blockIdx.y * src_stride_bytes;
-    float2* work = work0 + (size_t)blockIdx.y * pl.N;
+    const int f = blockIdx.y;
+    float2* work = work0 + (size_t)f * pl.N;
     const int col = threadIdx.x % C, t = threadIdx.x / C;
     const int n2 = blockIdx.x * C + col;
+    float2* const tws = smem + fr_smem_tiles<RA, RB>(C);      // [TW] coarse, then [N / TW] fine
+    float2* const fine = tws + pl.TW;
+    if (TAB) {
+        fr_stage_table(tws, pl.tw, pl.TW);
+        fr_stage_table(fine, pl.tw_fine, pl.N >> pl.logTW);
+    }
     float2 v[G::TP];
     if (t < RB) {
+        const FrameSrc fs = frame_src<FMT>(fr, f);
 #pragma unroll
-        for (int a = 0; a < RA; a++) { v[a] = load_windowed<FMT>(pl, src, (a * RB + t) * N2 + n2); }
+        for (int a = 0; a < RA; a++) { v[a] = load_frame<FMT>(pl, fs, (a * RB + t) * N2 + n2, !TAB); }
+        if (TAB) {
+            // window_p[(n2 RB + t) RA + a] = window[(a RB + t) N2 + n2], zero from nz on
+            const float4* __restrict__ wp = reinterpret_cast<const float4*>(pl.window_p + ((size_t)n2 * RB + t) * RA);
+#pragma unroll
+            for (int q = 0; q < RA / 4; q++) {
+                const float4 w = __ldg(wp + q);
+                v[4 * q + 0] = make_float2(v[4 * q + 0].x * w.x, v[4 * q + 0].y * w.x);
+                v[4 * q + 1] = make_float2(v[4 * q + 1].x * w.y, v[4 * q + 1].y * w.y);
+                v[4 * q + 2] = make_float2(v[4 * q + 2].x * w.z, v[4 * q + 2].y * w.z);
+                v[4 * q + 3] = make_float2(v[4 * q + 3].x * w.w, v[4 * q + 3].y * w.w);
+            }
+        }
     }
-    fr_transform<RA, RB>(v, smem + col * G::pitch, t, pl.tw, pl.logTW - pl.logN1);
+    if (TAB) { __syncthreads(); }
+    fr_transform<RA, RB, TAB>(v, smem + col * G::pitch, t, TAB ? tws : pl.tw, pl.logTW - pl.logN1);
     if (t < RA) {
         // W_N^(k1 n2) = coarse[(k1 n2) >> s] * fine[(k1 n2) & (2^s - 1)],  coarse = tw (unit 1/TW), fine unit 1/N
         const int s = pl.logN - pl.logTW;
@@ -111,7 +147,7 @@ __global__ void __launch_bounds__(C * FrGeom<RA, RB>::TP, MINB) k_fftr_p1(const 
         for (int d = 0; d < RB; d++) {
             const int k1 = t + RA * d;
             const unsigned e = (unsigned)k1 * (unsigned)n2;
-            const float2 w = cmulf(__ldg(pl.tw + (e >> s)), __ldg(pl.tw_fine + (e & msk)));
+            const float2 w = TAB ? cmulf(tws[e >> s], fine[e & msk]) : cmulf(__ldg(pl.tw + (e >> s)), __ldg(pl.tw_fine + (e & msk)));
             work[(size_t)k1 * N2 + n2] = cmulf(v[fr_brev<RB>(d)], w);
         }
     }
@@ -119,7 +155,8 @@ __global__ void __launch_bounds__(C * FrGeom<RA, RB>::TP, MINB) k_fftr_p1(const 
 
 // pass 2: CTA = R adjacent rows k1:  X[k1 + N1 k2] = sum_n2 A[k1][n2] W_N2^(n2 k2); dB epilogue, transposed through
 // shared memory so that the R rows' values of one k2 leave as one segment
-template <int RA, int RB, int R>
+// TAB: as in pass 1, the step-1 twiddles come from a shared-memory copy of tw
+template <int RA, int RB, int R, bool TAB>
 __global__ void __launch_bounds__(R * FrGeom<RA, RB>::TP) k_fftr_p2(const __grid_constant__ FftPlanDev pl, const float2* __restrict__ work0,
                                                                     float* __restrict__ out_db0) {
     using G = FrGeom<RA, RB>;
@@ -129,13 +166,16 @@ __global__ void __launch_bounds__(R * FrGeom<RA, RB>::TP) k_fftr_p2(const __grid
     float* out_db = out_db0 + (size_t)blockIdx.y * pl.N;
     const int t = threadIdx.x % G::TP, row = threadIdx.x / G::TP;
     const int r0 = blockIdx.x * R;
+    float2* const tws = smem + fr_smem_tiles<RA, RB>(R);
+    if (TAB) { fr_stage_table(tws, pl.tw, pl.TW); }
     float2 v[G::TP];
     if (t < RB) {
         const float2* __restrict__ p = work + (size_t)(r0 + row) * N2 + t;
 #pragma unroll
         for (int a = 0; a < RA; a++) { v[a] = __ldg(p + a * RB); }
     }
-    fr_transform<RA, RB>(v, smem + row * G::pitch, t, pl.tw, pl.logTW - pl.logN2);
+    if (TAB) { __syncthreads(); }
+    fr_transform<RA, RB, TAB>(v, smem + row * G::pitch, t, TAB ? tws : pl.tw, pl.logTW - pl.logN2);
     __syncthreads();                                    // every exchange tile has been read: reuse the space
     float* T = reinterpret_cast<float*>(smem);          // [k2][R + 1]
     const float nf = 1.0f / ((float)pl.N * (float)pl.N);

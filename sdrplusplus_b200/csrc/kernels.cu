@@ -565,25 +565,34 @@ __device__ __forceinline__ float power_db(float2 X, float normFactSq) {
     return l * 3.01029995663981209120f;
 }
 
+// frame f of a batch (FftFrames) as two bases: its sample n is at lo[n] for n < lim (the staged part), at hi[n] from lim on
+struct FrameSrc { const char* lo; const char* hi; int lim; };
 template <int FMT>
-__device__ __forceinline__ float2 load_windowed(const FftPlanDev& pl, const void* __restrict__ src, int n) {
+__device__ __forceinline__ FrameSrc frame_src(const FftFrames& fr, int f) {
+    constexpr int bps = FMT == FMT_CF32 ? 8 : (FMT == FMT_CS16 ? 4 : 2);
+    return { reinterpret_cast<const char*>(fr.pre), reinterpret_cast<const char*>(fr.chunk) + ((long long)f * fr.stride - fr.split) * bps,
+             f == 0 ? fr.split : 0 };
+}
+// sample n of a frame, zero from nz on; windowed: times window[n]
+template <int FMT>
+__device__ __forceinline__ float2 load_frame(const FftPlanDev& pl, const FrameSrc& fs, int n, bool windowed) {
     if (n >= pl.nz) { return make_float2(0.0f, 0.0f); }    // zero padding [nz, N)  (iq_frontend.cpp:301)
-    float2 x = load_iq<FMT>(src, n, pl.in_scale);
-    float w = __ldg(pl.window + n);
+    const float2 x = load_iq<FMT>(n < fs.lim ? fs.lo : fs.hi, n, pl.in_scale);
+    if (!windowed) { return x; }
+    const float w = __ldg(pl.window + n);
     return make_float2(x.x * w, x.y * w);
 }
 
 // single-pass: the whole transform fits one CTA's shared memory
 template <int FMT>
-__global__ void __launch_bounds__(512) k_fft_single(const __grid_constant__ FftPlanDev pl, const void* __restrict__ src0,
-                                                      float* __restrict__ out_db0, float2* __restrict__ out_raw,
-                                                      long long src_stride_bytes) {
+__global__ void __launch_bounds__(512) k_fft_single(const __grid_constant__ FftPlanDev pl, const __grid_constant__ FftFrames fr,
+                                                      float* __restrict__ out_db0, float2* __restrict__ out_raw) {
     extern __shared__ __align__(16) float2 smem[];
     const int N = pl.N;
-    const void* src = reinterpret_cast<const char*>(src0) + (size_t)blockIdx.y * src_stride_bytes;
     float* out_db = out_db0 + (size_t)blockIdx.y * N;
+    const FrameSrc fs = frame_src<FMT>(fr, blockIdx.y);
 #pragma unroll 4
-    for (int i = threadIdx.x; i < N; i += blockDim.x) { smem[padf(i)] = load_windowed<FMT>(pl, src, i); }
+    for (int i = threadIdx.x; i < N; i += blockDim.x) { smem[padf(i)] = load_frame<FMT>(pl, fs, i, true); }
     __syncthreads();
     fft_dif_smem<false>(smem, pl.logN, 1, N, pl.tw, pl.logTW);
     const float nf = 1.0f / ((float)N * (float)N);
@@ -597,17 +606,17 @@ __global__ void __launch_bounds__(512) k_fft_single(const __grid_constant__ FftP
 // pass 1 of the two-pass (four-step) transform: n = n1*N2 + n2, k = k1 + N1*k2.
 // CTA = C adjacent columns n2, all rows n1: A[k1][n2] = W_N^(k1*n2) * sum_n1 x[n1*N2+n2] W_N1^(n1*k1)
 template <int FMT>
-__global__ void __launch_bounds__(512) k_fft_p1(const __grid_constant__ FftPlanDev pl, const void* __restrict__ src0,
-                                                  float2* __restrict__ work0, int C, long long src_stride_bytes) {
+__global__ void __launch_bounds__(512) k_fft_p1(const __grid_constant__ FftPlanDev pl, const __grid_constant__ FftFrames fr,
+                                                  float2* __restrict__ work0, int C) {
     extern __shared__ __align__(16) float2 smem[];
     const int N1 = pl.N1, N2 = pl.N2;
-    const void* src = reinterpret_cast<const char*>(src0) + (size_t)blockIdx.y * src_stride_bytes;
     float2* work = work0 + (size_t)blockIdx.y * pl.N;
     const int c0 = blockIdx.x * C;
+    const FrameSrc fs = frame_src<FMT>(fr, blockIdx.y);
 #pragma unroll 4
     for (int t = threadIdx.x; t < N1 * C; t += blockDim.x) {
         int n1 = t / C, c = t - n1 * C;
-        smem[padf(t)] = load_windowed<FMT>(pl, src, n1 * N2 + c0 + c);
+        smem[padf(t)] = load_frame<FMT>(pl, fs, n1 * N2 + c0 + c, true);
     }
     __syncthreads();
     fft_dif_smem<true>(smem, pl.logN1, C, 0, pl.tw, pl.logTW);
@@ -1212,37 +1221,56 @@ cudaError_t launch_carry(const CarryParams& p, cudaStream_t s) {
     return launch_chain(k_carry, dim3((unsigned)p.njobs), dim3(256), 0, s, p);
 }
 
+bool fft_plan_uses_reg(const FftPlanDev& pl) {
+    return pl.N2 > 1 && pl.logN1 >= 8 && pl.logN1 <= 10 && pl.logN2 >= 8 && pl.logN2 <= 10;
+}
+
 template <int FMT>
-static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const void* src, float2* work, float* out_db, float2* out_raw,
-                                  cudaStream_t s, int* nlaunch, int nbatch, long long src_stride_bytes) {
+static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const FftFrames& fr, float2* work, float* out_db, float2* out_raw,
+                                  cudaStream_t s, int* nlaunch, bool tables) {
     cudaError_t e;
+    const int nbatch = fr.nbatch;
     if (pl.N1 == pl.N) {
         size_t smem = ((size_t)pl.N + (pl.N >> 4) + 2) * sizeof(float2);
         e = set_smem(k_fft_single<FMT>, smem);
         if (e != cudaSuccess) { return e; }
         int thr = pl.N / 8 < 32 ? 32 : (pl.N / 8 > 512 ? 512 : pl.N / 8);
-        k_fft_single<FMT><<<dim3(1, nbatch), thr, smem, s>>>(pl, src, out_db, out_raw, src_stride_bytes);
+        k_fft_single<FMT><<<dim3(1, nbatch), thr, smem, s>>>(pl, fr, out_db, out_raw);
         if (nlaunch) { (*nlaunch)++; }
         return cudaGetLastError();
     }
     // two passes
-    if (g_fft_variant >= 1 && !out_raw && pl.tw_fine && pl.logN1 >= 8 && pl.logN1 <= 10 && pl.logN2 >= 8 && pl.logN2 <= 10) {
+    if (g_fft_variant >= 1 && !out_raw && pl.tw_fine && pl.window_p && fft_plan_uses_reg(pl)) {
         // register-resident column / row transforms (fft_reg.cuh)
-        // transforms per CTA: 8 (256 threads, 69 KB) or 4 (128 threads, 34 KB: at 128 registers a thread, a CTA of four still
-        // fits on an SM beside stage 1's persistent CTA AND a CTA of the chain behind it -- kernels_set_fft_cta)
+        // transforms per CTA: 8 (256 threads) or 4 (128 threads) -- kernels_set_fft_cta; DESIGN.md section 4 has the residency.
+        // tables: + TW + N/TW float2 of twiddles in shared memory (pass 1), + TW (pass 2)
 #define FR_P1(RA, RB, CC)                                                                                      \
         do {                                                                                                   \
-            const size_t sm = (size_t)CC * FrGeom<RA, RB>::pitch * sizeof(float2);                             \
-            e = set_smem(k_fftr_p1<FMT, RA, RB, CC, 2>, sm);                                                   \
-            if (e != cudaSuccess) { return e; }                                                                \
-            k_fftr_p1<FMT, RA, RB, CC, 2><<<dim3(pl.N2 / CC, nbatch), CC * FrGeom<RA, RB>::TP, sm, s>>>(pl, src, work, src_stride_bytes); \
+            const size_t sm = (fr_smem_tiles<RA, RB>(CC) + (tables ? (size_t)pl.TW + (pl.N >> pl.logTW) : 0)) * sizeof(float2); \
+            if (tables) {                                                                                      \
+                e = set_smem(k_fftr_p1<FMT, RA, RB, CC, true>, sm);                                         \
+                if (e != cudaSuccess) { return e; }                                                            \
+                k_fftr_p1<FMT, RA, RB, CC, true><<<dim3(pl.N2 / CC, nbatch), CC * FrGeom<RA, RB>::TP, sm, s>>>(pl, fr, work); \
+            }                                                                                                  \
+            else {                                                                                             \
+                e = set_smem(k_fftr_p1<FMT, RA, RB, CC, false>, sm);                                        \
+                if (e != cudaSuccess) { return e; }                                                            \
+                k_fftr_p1<FMT, RA, RB, CC, false><<<dim3(pl.N2 / CC, nbatch), CC * FrGeom<RA, RB>::TP, sm, s>>>(pl, fr, work); \
+            }                                                                                                  \
         } while (0)
 #define FR_P2(RA, RB, RR)                                                                                      \
         do {                                                                                                   \
-            const size_t sm = (size_t)RR * FrGeom<RA, RB>::pitch * sizeof(float2);                             \
-            e = set_smem(k_fftr_p2<RA, RB, RR>, sm);                                                           \
-            if (e != cudaSuccess) { return e; }                                                                \
-            k_fftr_p2<RA, RB, RR><<<dim3(pl.N1 / RR, nbatch), RR * FrGeom<RA, RB>::TP, sm, s>>>(pl, work, out_db); \
+            const size_t sm = (fr_smem_tiles<RA, RB>(RR) + (tables ? (size_t)pl.TW : 0)) * sizeof(float2);     \
+            if (tables) {                                                                                      \
+                e = set_smem(k_fftr_p2<RA, RB, RR, true>, sm);                                                 \
+                if (e != cudaSuccess) { return e; }                                                            \
+                k_fftr_p2<RA, RB, RR, true><<<dim3(pl.N1 / RR, nbatch), RR * FrGeom<RA, RB>::TP, sm, s>>>(pl, work, out_db); \
+            }                                                                                                  \
+            else {                                                                                             \
+                e = set_smem(k_fftr_p2<RA, RB, RR, false>, sm);                                                \
+                if (e != cudaSuccess) { return e; }                                                            \
+                k_fftr_p2<RA, RB, RR, false><<<dim3(pl.N1 / RR, nbatch), RR * FrGeom<RA, RB>::TP, sm, s>>>(pl, work, out_db); \
+            }                                                                                                  \
         } while (0)
         if (g_fft_cta == 4) {
             if (pl.logN1 == 10) { FR_P1(32, 32, 4); } else if (pl.logN1 == 9) { FR_P1(16, 32, 4); } else { FR_P1(16, 16, 4); }
@@ -1279,7 +1307,7 @@ static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const void* src, float2*
     e = set_smem(k_fft_p2, smem2);
     if (e != cudaSuccess) { return e; }
     const int thr1 = (pl.N1 / 8) * C >= 512 ? 512 : 256, thr2 = (pl.N2 / 8) * R >= 512 ? 512 : 256;
-    k_fft_p1<FMT><<<dim3(pl.N2 / C, nbatch), thr1, smem1, s>>>(pl, src, work, C, src_stride_bytes);
+    k_fft_p1<FMT><<<dim3(pl.N2 / C, nbatch), thr1, smem1, s>>>(pl, fr, work, C);
     e = cudaGetLastError();
     if (e != cudaSuccess) { return e; }
     k_fft_p2<<<dim3(pl.N1 / R, nbatch), thr2, smem2, s>>>(pl, work, out_db, out_raw, R);
@@ -1287,16 +1315,17 @@ static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const void* src, float2*
     return cudaGetLastError();
 }
 
-cudaError_t launch_fft_frames(const FftPlanDev& pl, const void* src, int fmt, float2* work, float* out_db,
-                              float2* out_raw, cudaStream_t s, int* nlaunch, int nbatch, long long src_stride_bytes) {
-    if (nbatch <= 0) { return cudaSuccess; }
-    if (fmt == FMT_CF32) { return launch_fft_fmt<FMT_CF32>(pl, src, work, out_db, out_raw, s, nlaunch, nbatch, src_stride_bytes); }
-    if (fmt == FMT_CS16) { return launch_fft_fmt<FMT_CS16>(pl, src, work, out_db, out_raw, s, nlaunch, nbatch, src_stride_bytes); }
-    return launch_fft_fmt<FMT_CS8>(pl, src, work, out_db, out_raw, s, nlaunch, nbatch, src_stride_bytes);
+cudaError_t launch_fft_frames(const FftPlanDev& pl, const FftFrames& fr, int fmt, float2* work, float* out_db,
+                              float2* out_raw, cudaStream_t s, int* nlaunch, bool tables) {
+    if (fr.nbatch <= 0) { return cudaSuccess; }
+    if (fmt == FMT_CF32) { return launch_fft_fmt<FMT_CF32>(pl, fr, work, out_db, out_raw, s, nlaunch, tables); }
+    if (fmt == FMT_CS16) { return launch_fft_fmt<FMT_CS16>(pl, fr, work, out_db, out_raw, s, nlaunch, tables); }
+    return launch_fft_fmt<FMT_CS8>(pl, fr, work, out_db, out_raw, s, nlaunch, tables);
 }
 cudaError_t launch_fft_frame(const FftPlanDev& pl, const void* src, int fmt, float2* work, float* out_db,
                              float2* out_raw, cudaStream_t s, int* nlaunch) {
-    return launch_fft_frames(pl, src, fmt, work, out_db, out_raw, s, nlaunch, 1, 0);
+    const FftFrames fr{ src, nullptr, 0, 0, 1 };
+    return launch_fft_frames(pl, fr, fmt, work, out_db, out_raw, s, nlaunch, true);
 }
 
 cudaError_t launch_convert_cf32(const void* src, int fmt, float2* dst, int n, float scale, cudaStream_t s) {

@@ -339,6 +339,7 @@ struct FftPlanDev {
     int TW, logTW;
     const float2* tw_fine;  // exp(-2 pi i j / N), j < N / TW (two-pass plans; null otherwise)
     const float* window;    // nz floats: window(i,nz) * (-1)^i
+    const float* window_p;  // register-FFT plans: window in pass 1's per-thread order (fft_reg.cuh), zero from nz on; else null
     float in_scale;         // integer input formats: sample = (float)x * in_scale
     int nz;
 };
@@ -356,12 +357,25 @@ cudaError_t launch_seq(const SeqParams& p, cudaStream_t s);
 cudaError_t launch_m2s(const M2SParams& p, cudaStream_t s);
 cudaError_t launch_scale(const ScaleParams& p, cudaStream_t s);
 cudaError_t launch_carry(const CarryParams& p, cudaStream_t s);
+// Where a batch of frames comes from: frame f's sample n is chunk[f * stride + n - split] (format fmt, index in samples).
+// split > 0 only for a frame that began in earlier chunks: its first split samples were staged, in the same format, at
+// pre[0 .. split), and chunk points at the first sample of this chunk.
+struct FftFrames {
+    const void* chunk;
+    const void* pre;
+    long long stride;
+    int split;
+    int nbatch;
+};
 // src: nz samples of format fmt (chunk data), read directly; out_db: N floats; work: N float2 scratch
 cudaError_t launch_fft_frame(const FftPlanDev& pl, const void* src, int fmt, float2* work, float* out_db,
                              float2* out_raw, cudaStream_t s, int* nlaunch);
-// nbatch equally spaced frames (src_stride_bytes apart) in one launch pair; work: nbatch*N float2, out_db: nbatch*N
-cudaError_t launch_fft_frames(const FftPlanDev& pl, const void* src, int fmt, float2* work, float* out_db,
-                              float2* out_raw, cudaStream_t s, int* nlaunch, int nbatch, long long src_stride_bytes);
+// fr.nbatch frames in one launch pair; work: nbatch*N float2, out_db: nbatch*N.  tables: the register passes stage their
+// twiddle tables in shared memory and read the window as vectors (same values, same output bits); false = global gathers
+cudaError_t launch_fft_frames(const FftPlanDev& pl, const FftFrames& fr, int fmt, float2* work, float* out_db,
+                              float2* out_raw, cudaStream_t s, int* nlaunch, bool tables);
+// the register passes serve this plan (pass-1 window order: window_p)
+bool fft_plan_uses_reg(const FftPlanDev& pl);
 // IQFrontEnd pre-processing at the input rate: DC blocker + conjugate (preproc.cuh)
 struct DcbParams {
     const void* in;          // chunk (format fmt)
