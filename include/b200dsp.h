@@ -217,6 +217,17 @@ int b200_fe_remove_vfo(b200_fe* fe, int id);
 /* RxVFO::setOffset / setBandwidth (core/src/dsp/channel/rx_vfo.h:60-77): phase-continuous, next chunk */
 int b200_fe_set_vfo_offset(b200_fe* fe, int id, double offset);
 int b200_fe_set_vfo_bandwidth(b200_fe* fe, int id, double bandwidth);
+/* radio_module.h setters: the VFO takes cfg at the next chunk boundary, keeping state as the reference's setters do.
+ * Checked whole at the call (B200_EINVAL leaves the VFO as it was), stored, and applied by the first submit / process after
+ * it; of several calls before one chunk the last wins.  offset / bandwidth: as b200_fe_set_vfo_offset / _bandwidth -- and, the
+ * last call winning, a cfg.offset / cfg.bandwidth equal to the VFO's applied value cancels an earlier set_vfo_offset / _bandwidth.
+ * Coefficients keep the block's state: af_volume, af_muted, squelch_level, nb_level, agc_attack, agc_decay, dc_block_rate
+ * (AM), af_deemph_tau non-zero -> non-zero.  agc_mode (AM) restarts the AM demodulator's AGCs and DC blocker, nr_bins the
+ * FM IF noise reduction.  nb_on, squelch_on, nr_on, af_high_pass, af_deemph_tau 0 <-> non-zero and af_volume_on switch a
+ * block on or off (chain::setBlockEnabled): the other blocks keep their state, a block switched off keeps its own and goes
+ * on from it when switched on again (b200_fe_reset clears it).  demod, out_samplerate, deviation, low_pass and
+ * af_samplerate need a new demodulator: B200_EINVAL (remove the VFO and add it again).  Output counts never change. */
+int b200_fe_set_vfo_config(b200_fe* fe, int id, const b200_vfo_cfg* cfg);
 int b200_fe_vfo_count(b200_fe* fe);
 /* upper bound of output samples one chunk of `count` input samples can produce for VFO id */
 int b200_fe_vfo_max_out(b200_fe* fe, int id, int count);

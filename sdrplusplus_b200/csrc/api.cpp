@@ -233,12 +233,24 @@ int RdsCore::reset(cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------ front end
+// Stage::role of a VFO's stages: the radio blocks b200_fe_set_vfo_config switches on and off, in chain order (IF chain behind the
+// channel filter, AF chain at the end), and the AM / SSB demodulator stage whose AGC it retunes
+enum VfoRole { ROLE_NONE = 0, ROLE_NB, ROLE_SQUELCH, ROLE_NR, ROLE_HPF, ROLE_DEEMPH, ROLE_VOLUME, ROLE_DEMOD, ROLE_COUNT };
+static bool role_in_if_chain(int r) { return r >= ROLE_NB && r <= ROLE_NR; }
+static bool role_in_af_chain(int r) { return r >= ROLE_HPF && r <= ROLE_VOLUME; }
+
 struct VfoSlot {
     bool used = false;
     b200_vfo_cfg cfg;
     Chain chain;
     bool pend_offset = false, pend_bw = false;
     double new_offset = 0, new_bw = 0;
+    // b200_fe_set_vfo_config: the config taken at the next chunk boundary, and the blocks switched off by an earlier call,
+    // parked with their state (chain::setBlockEnabled keeps a disabled block as it was)
+    bool pend_cfg = false;
+    b200_vfo_cfg new_cfg;
+    std::unique_ptr<Stage> parked[ROLE_COUNT];
+    bool hpf_at_add = false;     // b200_fe_vfo_max_out counts the high-pass FIR's spare output (FirCStage::max_out) when add built it
     // B200_DEMOD_WFM_RDS_BITS: RDSDemod behind the chain, and where its records wait for the copy to a host buffer
     std::unique_ptr<RdsCore> rds;
     DevBuf rds_rec;
@@ -459,14 +471,29 @@ extern "C" int b200_fe_set_fft(b200_fe* fe, int size, double rate, int window) {
     return 0;
 }
 
+// the AF chain and the volume follow audio only
+static bool vfo_has_audio(const b200_vfo_cfg& c) {
+    return c.demod != B200_DEMOD_RAW && c.demod != B200_DEMOD_WFM_RDS && c.demod != B200_DEMOD_WFM_RDS_BITS;
+}
+
 static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
     const b200_vfo_cfg& c = v->cfg;
     int rc = v->chain.add_rxvfo(fe->fs_eff, c.out_samplerate, c.bandwidth, c.offset);
     if (rc) { return rc; }
     // radio IF chain (radio_module.h:94-96): noise blanker -> power squelch -> FM IF noise reduction
-    if (c.nb_on && (rc = v->chain.add_noise_blanker(500.0 / c.out_samplerate, c.nb_level))) { return rc; }
-    if (c.squelch_on && (rc = v->chain.add_squelch(c.squelch_level))) { return rc; }
-    if (c.nr_on && (rc = v->chain.add_fmif(c.nr_bins))) { return rc; }
+    auto& st = v->chain.st;
+    if (c.nb_on) {
+        if ((rc = v->chain.add_noise_blanker(500.0 / c.out_samplerate, c.nb_level))) { return rc; }
+        st.back()->role = ROLE_NB;
+    }
+    if (c.squelch_on) {
+        if ((rc = v->chain.add_squelch(c.squelch_level))) { return rc; }
+        st.back()->role = ROLE_SQUELCH;
+    }
+    if (c.nr_on) {
+        if ((rc = v->chain.add_fmif(c.nr_bins))) { return rc; }
+        st.back()->role = ROLE_NR;
+    }
     switch (c.demod) {
     case B200_DEMOD_RAW: break;
     case B200_DEMOD_WFM: rc = v->chain.add_wfm(c.deviation, c.out_samplerate, c.low_pass != 0, false); break;
@@ -481,12 +508,17 @@ static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
     default: set_error("unknown demodulator %d", c.demod); return B200_EINVAL;
     }
     if (rc) { return rc; }
-    const bool audio = c.demod != B200_DEMOD_RAW && c.demod != B200_DEMOD_WFM_RDS && c.demod != B200_DEMOD_WFM_RDS_BITS;     // the AF chain and the volume follow audio only
+    if (c.demod >= B200_DEMOD_AM && c.demod <= B200_DEMOD_DSB) { st[st.size() - 2]->role = ROLE_DEMOD; }    // AGC stage, then low-pass / M2S
+    const bool audio = vfo_has_audio(c);
     if (c.af_samplerate > 0 && audio) {
         if ((rc = v->chain.add_af_chain(c.out_samplerate, c.af_samplerate, c.af_high_pass != 0, c.af_deemph_tau))) { return rc; }
+        size_t k = st.size();
+        if (c.af_deemph_tau > 0.0) { st[--k]->role = ROLE_DEEMPH; }
+        if (c.af_high_pass) { st[--k]->role = ROLE_HPF; v->hpf_at_add = true; }
     }
     if (c.af_volume_on && audio) {
         if ((rc = v->chain.add_volume(c.af_volume, c.af_muted != 0))) { return rc; }
+        st.back()->role = ROLE_VOLUME;
     }
     const bool ov = fe->sch.tail_stream != nullptr;
     if (ov && v->chain.st.size() == 1) {
@@ -508,7 +540,11 @@ static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
 
 // what one chunk of `count` samples can put into a VFO's output buffer, in 8-byte elements
 static int vfo_out_bound(const VfoSlot* v, int count) {
-    const int n = v->chain.max_out(count);
+    int n = v->chain.max_out(count);
+    // the high-pass FIR is 1:1 but its bound has a spare output: whether b200_fe_set_vfo_config switched it on or off since, the
+    // bound stays the one b200_fe_add_vfo gave
+    for (auto& s : v->chain.st) { n -= s->role == ROLE_HPF ? 1 : 0; }
+    n += v->hpf_at_add ? 1 : 0;
     return v->rds ? b200_rds_demod_max_out(n) : n;
 }
 
@@ -566,6 +602,35 @@ extern "C" int b200_fe_set_vfo_bandwidth(b200_fe* fe, int id, double bw) {
     if (!v || bw <= 0) { set_error("bad bandwidth"); return B200_EINVAL; }
     v->pend_bw = true;
     v->new_bw = bw;
+    return 0;
+}
+// the radio module's setters (radio_module.h:606-760) between chunks: checked here, taken whole by apply_pending
+extern "C" int b200_fe_set_vfo_config(b200_fe* fe, int id, const b200_vfo_cfg* cfg) {
+    if (!fe || !cfg) { set_error("null argument"); return B200_EINVAL; }
+    std::lock_guard<std::mutex> lck(fe->mtx);
+    VfoSlot* v = get_vfo(fe, id);
+    if (!v) { return B200_EINVAL; }
+    const b200_vfo_cfg& o = v->cfg;
+    const char* field = cfg->demod != o.demod ? "demod" : cfg->out_samplerate != o.out_samplerate ? "out_samplerate" :
+                        cfg->deviation != o.deviation ? "deviation" : cfg->low_pass != o.low_pass ? "low_pass" :
+                        cfg->af_samplerate != o.af_samplerate ? "af_samplerate" : nullptr;
+    if (field) {
+        set_error("VFO %d: %s needs a new demodulator or AF resampler: remove the VFO and add it again", id, field);
+        return B200_EINVAL;
+    }
+    if (cfg->bandwidth <= 0) { set_error("bad bandwidth"); return B200_EINVAL; }
+    if (o.demod == B200_DEMOD_AM && cfg->agc_mode != B200_AGC_CARRIER && cfg->agc_mode != B200_AGC_AUDIO) { set_error("bad AM agc_mode"); return B200_EINVAL; }
+    if (cfg->nr_on && !fmif_supported(cfg->nr_bins)) {
+        set_error("FM IF noise reduction: %d bins (supported: 2 ... %d)", cfg->nr_bins, 64);
+        return B200_EINVAL;
+    }
+    // offset and bandwidth go the way of b200_fe_set_vfo_offset / _bandwidth; the last call before a chunk wins
+    v->pend_offset = cfg->offset != o.offset;
+    v->new_offset = cfg->offset;
+    v->pend_bw = cfg->bandwidth != o.bandwidth;
+    v->new_bw = cfg->bandwidth;
+    v->new_cfg = *cfg;
+    v->pend_cfg = true;
     return 0;
 }
 extern "C" int b200_fe_vfo_count(b200_fe* fe) {
@@ -670,7 +735,9 @@ extern "C" int b200_fe_reset(b200_fe* fe) {
     for (auto& v : fe->vfos) {
         if (v->used) { v->chain.reset_state(); }
         if (v->used && v->rds) { int rcr = v->rds->reset(nullptr); if (rcr) { return rcr; } }
+        for (auto& p : v->parked) { if (p) { clear_stage_state(*p); } }     // a block switched on later starts fresh
     }
+    B200_CK(cudaDeviceSynchronize());
     int rc = fe->sch.reset_raw();
     if (!fe->pre.st.empty()) { fe->pre.reset_state(); }
     if (fe->dc_state.p) { B200_CK(cudaMemset(fe->dc_state.p, 0, 16)); B200_CK(cudaDeviceSynchronize()); }
@@ -695,11 +762,146 @@ static inline long long host_clock_ns() {
     return (long long)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
-// apply RxVFO::setOffset / setBandwidth at the chunk boundary (rx_vfo.h:60-77)
-static void apply_pending(b200_fe* fe) {
+// A VFO's stages with the IF / AF blocks in `order` and the switched-off blocks in `parked`.  Every stage comes from the chain,
+// the parked slots or `pool`; what is left over goes to `pool`.
+static void place_stages(VfoSlot* v, const std::vector<Stage*>& order, Stage* const* parked, std::vector<std::unique_ptr<Stage>>& pool) {
+    for (auto& s : v->chain.st) { pool.push_back(std::move(s)); }
+    for (auto& p : v->parked) { if (p) { pool.push_back(std::move(p)); } }
+    v->chain.st.clear();
+    auto take = [&](Stage* s) {
+        std::unique_ptr<Stage> u;
+        for (auto& q : pool) { if (q.get() == s) { u = std::move(q); break; } }
+        return u;
+    };
+    for (Stage* s : order) { v->chain.st.push_back(take(s)); }
+    for (int r = 0; r < ROLE_COUNT; r++) { if (parked[r]) { v->parked[r] = take(parked[r]); } }
+    pool.erase(std::remove(pool.begin(), pool.end(), nullptr), pool.end());
+}
+
+// b200_fe_set_vfo_config at the chunk boundary.  Coefficients: the host-side parameters the next launch list carries (no device
+// wait).  AGC mode (AM::setAGCMode -> reset, am.h:49-56) and bin count (FMIF::setBins, fm_if.h:26-34): that block restarts.
+// Blocks switched on / off: chain::setBlockEnabled (chain.h:61-127) -- the other stages keep their buffers and state, a block
+// switched off is parked as it is and carries on from there when switched on again.  On an error the VFO is left as it was.
+static int apply_vfo_config(VfoSlot* v, const b200_vfo_cfg& n) {
+    const b200_vfo_cfg& o = v->cfg;
+    Chain& ch = v->chain;
+    const bool audio = vfo_has_audio(o), af = audio && o.af_samplerate > 0;
+    bool want[ROLE_COUNT] = {};
+    want[ROLE_NB] = n.nb_on != 0;
+    want[ROLE_SQUELCH] = n.squelch_on != 0;
+    want[ROLE_NR] = n.nr_on != 0;
+    want[ROLE_HPF] = af && n.af_high_pass;
+    want[ROLE_DEEMPH] = af && n.af_deemph_tau > 0.0;
+    want[ROLE_VOLUME] = audio && n.af_volume_on;
+    Stage* live[ROLE_COUNT] = {};
+    for (auto& s : ch.st) { if (s->role) { live[s->role] = s.get(); } }
+    const bool new_bins = n.nr_bins != o.nr_bins;            // FMIF::setBins: the block restarts with the new bin count
+    bool topo = new_bins && (live[ROLE_NR] || v->parked[ROLE_NR]);
+    for (int r = ROLE_NB; r <= ROLE_VOLUME; r++) { topo = topo || want[r] != (live[r] != nullptr); }
+    const bool am_restart = o.demod == B200_DEMOD_AM && n.agc_mode != o.agc_mode && live[ROLE_DEMOD];
+    if (topo || am_restart) { B200_CK(cudaDeviceSynchronize()); }     // chunks in flight still read the stages
+    if (topo) {
+        // new stages first: nothing has changed when one of them fails
+        std::unique_ptr<Stage> fresh[ROLE_COUNT];
+        const size_t after_chan = (size_t)ch.chan_fir + 1;
+        const int if_cap = after_chan < ch.st.size() ? ch.st[after_chan]->cap_in : ch.out_cap;    // every toggled block is 1:1
+        for (int r = ROLE_NB; r <= ROLE_VOLUME; r++) {
+            const bool reuse = (live[r] || v->parked[r]) && !(r == ROLE_NR && new_bins);
+            if (!want[r] || reuse) { continue; }
+            Chain tmp;
+            int rc = 0;
+            switch (r) {
+            case ROLE_NB: rc = tmp.add_noise_blanker(500.0 / o.out_samplerate, n.nb_level); break;
+            case ROLE_SQUELCH: rc = tmp.add_squelch(n.squelch_level); break;
+            case ROLE_NR: rc = tmp.add_fmif(n.nr_bins); break;
+            case ROLE_HPF: rc = tmp.add_af_highpass(o.af_samplerate); break;
+            case ROLE_DEEMPH: rc = tmp.add_deemph(n.af_deemph_tau, o.af_samplerate); break;
+            default: rc = tmp.add_volume(n.af_volume, n.af_muted != 0); break;
+            }
+            if (rc) { return rc; }
+            fresh[r] = std::move(tmp.st[0]);
+            fresh[r]->role = r;
+            if (r == ROLE_VOLUME) { fresh[r]->in_es = fresh[r]->out_es = ch.out_es; }
+            if ((rc = fresh[r]->alloc_in(role_in_if_chain(r) ? if_cap : ch.out_cap))) { return rc; }
+        }
+        auto pick = [&](int r) -> Stage* {
+            if (!want[r]) { return nullptr; }
+            if (fresh[r]) { return fresh[r].get(); }
+            return live[r] ? live[r] : v->parked[r].get();
+        };
+        // the new order: IF blocks right behind the channel filter, AF blocks at the end, as build_vfo_chain places them
+        std::vector<Stage*> order, old_order;
+        Stage* parked[ROLE_COUNT] = {};
+        Stage* old_parked[ROLE_COUNT] = {};
+        for (size_t i = 0; i < ch.st.size(); i++) {
+            Stage* s = ch.st[i].get();
+            old_order.push_back(s);
+            if (!role_in_if_chain(s->role) && !role_in_af_chain(s->role)) { order.push_back(s); }
+            if ((int)i == ch.chan_fir) {
+                for (int r = ROLE_NB; r <= ROLE_NR; r++) { if (pick(r)) { order.push_back(pick(r)); } }
+            }
+        }
+        for (int r = ROLE_HPF; r <= ROLE_VOLUME; r++) { if (pick(r)) { order.push_back(pick(r)); } }
+        for (int r = ROLE_NB; r <= ROLE_VOLUME; r++) {
+            old_parked[r] = v->parked[r].get();
+            if (!want[r] && !(r == ROLE_NR && new_bins)) { parked[r] = live[r] ? live[r] : v->parked[r].get(); }
+        }
+        std::vector<std::unique_ptr<Stage>> pool;
+        for (auto& f : fresh) { if (f) { pool.push_back(std::move(f)); } }
+        int rc = ch.unfuse_history();
+        if (!rc) {
+            place_stages(v, order, parked, pool);
+            rc = ch.restage();
+            if (rc) {
+                place_stages(v, old_order, old_parked, pool);
+                int rc2 = ch.restage();
+                if (rc2) { return rc2; }
+            }
+        }
+        if (rc) { return rc; }
+    }
+    // coefficients, on the running and on the parked stages
+    auto coef = [&](Stage* s) {
+        switch (s->role) {
+        case ROLE_NB: ((SeqStage*)s)->proto.nb_level = (float)n.nb_level; break;                 // NoiseBlanker::setLevel
+        case ROLE_SQUELCH: ((SquelchStage*)s)->level = (float)n.squelch_level; break;             // PowerSquelch::setLevel
+        case ROLE_DEEMPH: if (n.af_deemph_tau > 0.0) { ((SeqStage*)s)->set_deemph_tau(n.af_deemph_tau, o.af_samplerate); } break;
+        case ROLE_VOLUME: ((ScaleStage*)s)->gain = n.af_muted ? 0.0f : powf((float)n.af_volume, 2); break;   // Volume::setVolume / setMuted
+        case ROLE_DEMOD: {
+            SeqStage* q = (SeqStage*)s;
+            q->set_agc(n.agc_attack, n.agc_decay);                                                   // AM / SSB setAGCAttack / setAGCDecay
+            if (o.demod == B200_DEMOD_AM) { q->proto.dc_rate = (float)n.dc_block_rate; q->proto.agc_mode = n.agc_mode; }   // setDCBlockRate
+            break;
+        }
+        default: break;
+        }
+    };
+    for (auto& s : ch.st) { coef(s.get()); }
+    for (auto& p : v->parked) { if (p) { coef(p.get()); } }
+    if (am_restart) {
+        // AM::reset: both AGCs and the DC blocker start over; the audio low-pass keeps its delay line
+        SeqStage* q = nullptr;
+        for (auto& s : ch.st) { if (s->role == ROLE_DEMOD) { q = (SeqStage*)s.get(); } }
+        B200_CK(cudaMemcpy(q->state.p, q->init_state, sizeof(q->init_state), cudaMemcpyHostToDevice));
+        B200_CK(cudaDeviceSynchronize());      // legacy-stream copy: done before the library's streams go on
+    }
+    const double off = v->cfg.offset, bw = v->cfg.bandwidth;      // routed through pend_offset / pend_bw
+    v->cfg = n;
+    v->cfg.offset = off;
+    v->cfg.bandwidth = bw;
+    return 0;
+}
+
+// apply RxVFO::setOffset / setBandwidth at the chunk boundary (rx_vfo.h:60-77), and b200_fe_set_vfo_config
+static int apply_pending(b200_fe* fe) {
     for (auto& up : fe->vfos) {
         VfoSlot* v = up.get();
         if (!v->used) { continue; }
+        if (v->pend_cfg) {
+            v->pend_cfg = false;
+            int rc = apply_vfo_config(v, v->new_cfg);
+            if (rc) { return rc; }
+        }
         if (v->pend_offset) {
             v->cfg.offset = v->new_offset;
             ((XdStage*)v->chain.st[0].get())->set_offset_rad(hz_to_rads(-v->cfg.offset, fe->fs_eff));
@@ -717,6 +919,7 @@ static void apply_pending(b200_fe* fe) {
             v->pend_bw = false;
         }
     }
+    return 0;
 }
 
 static int fe_fft_chunk(b200_fe* fe, const void* dptr, int fmt, int count, int* nlines) {
@@ -845,7 +1048,7 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
     if (fe->nsub - fe->nwait >= (unsigned long long)fe->max_inflight) { set_error("%d chunks already in flight: call b200_fe_wait", fe->max_inflight); return B200_ESTATE; }
     std::lock_guard<std::mutex> lck(fe->mtx);
     const long long hp0 = host_clock_ns();
-    apply_pending(fe);
+    { int rcp = apply_pending(fe); if (rcp) { return rcp; } }
     const int slot = (int)(fe->nsub % FE_SLOTS);
     cudaStream_t s = fe->sch.stream;
     const size_t in_bytes = (size_t)count * bytes_per_sample(in_fmt);

@@ -308,11 +308,21 @@ int SeqStage::configure_ssb(int mode, double bandwidth, double samplerate, doubl
     return 0;
 }
 
+void SeqStage::set_agc(double attack, double decay) {
+    proto.attack = (float)attack;
+    proto.inv_attack = 1.0f - proto.attack;
+    proto.decay = (float)decay;
+    proto.inv_decay = 1.0f - proto.decay;
+}
+void SeqStage::set_deemph_tau(double tau, double samplerate) {
+    float dt = 1.0f / samplerate;                       // deephasis.h:91-94: dt is a float
+    proto.alpha = dt / (tau + dt);
+}
+
 int SeqStage::configure_deemph(double tau, double samplerate) {
     memset(&proto, 0, sizeof(proto));
     proto.kind = 2;
-    float dt = 1.0f / samplerate;                       // deephasis.h:91-94: dt is a float
-    proto.alpha = dt / (tau + dt);
+    set_deemph_tau(tau, samplerate);
     in_es = 2;
     out_es = 2;
     memset(init_state, 0, sizeof(init_state));
@@ -566,22 +576,46 @@ int Chain::peek(int n) const {
     }
     return n;
 }
+void clear_stage_state(Stage& s) {
+    s.reset_state();
+    if (s.inbuf.p && s.hist > 0) { cudaMemset(s.inbuf.p, 0, (size_t)s.hist * s.in_es * sizeof(float)); }
+    if (s.inbuf_alt.p && s.hist > 0) { cudaMemset(s.inbuf_alt.p, 0, (size_t)s.hist * s.in_es * sizeof(float)); }
+    for (int i = 0; i < 2; i++) {
+        if (s.fh[i].p) { cudaMemset(s.fh[i].p, 0, s.fh[i].bytes); }
+    }
+    s.fpar = 0;
+    if (s.kind == K_SEQ) {
+        SeqStage* q = (SeqStage*)&s;
+        // AM::reset / AGC::reset (am.h:90-98, agc.h:64-68), Deemphasis::reset; the SSB demodulator has no reset
+        cudaMemcpy(q->state.p, q->init_state, sizeof(q->init_state), cudaMemcpyHostToDevice);
+    }
+}
 void Chain::reset_state() {
+    for (auto& s : st) { clear_stage_state(*s); }
+    cudaDeviceSynchronize();      // the memsets above run on the legacy stream: finish them before the library's streams go on
+}
+
+int Chain::unfuse_history() {
     for (auto& s : st) {
-        s->reset_state();
-        if (s->inbuf.p && s->hist > 0) { cudaMemset(s->inbuf.p, 0, (size_t)s->hist * s->in_es * sizeof(float)); }
-        if (s->inbuf_alt.p && s->hist > 0) { cudaMemset(s->inbuf_alt.p, 0, (size_t)s->hist * s->in_es * sizeof(float)); }
-        for (int i = 0; i < 2; i++) {
-            if (s->fh[i].p) { cudaMemset(s->fh[i].p, 0, s->fh[i].bytes); }
+        if (s->fmid && s->hist > 0) {
+            // a fused-middle stage is never the double-buffered stage behind stage 1: its plain history is the head of inbuf
+            B200_CK(cudaMemcpy(s->inbuf.p, s->fh[s->fpar].p, (size_t)s->hist * s->in_es * sizeof(float), cudaMemcpyDeviceToDevice));
         }
-        s->fpar = 0;
-        if (s->kind == K_SEQ) {
-            SeqStage* q = (SeqStage*)s.get();
-            // AM::reset / AGC::reset (am.h:90-98, agc.h:64-68), Deemphasis::reset; the SSB demodulator has no reset
-            cudaMemcpy(q->state.p, q->init_state, sizeof(q->init_state), cudaMemcpyHostToDevice);
+        s->fmid = false;
+    }
+    B200_CK(cudaDeviceSynchronize());
+    return 0;
+}
+int Chain::restage() {
+    int rc = plan_fused();
+    if (rc) { return rc; }
+    for (auto& s : st) {
+        if (s->fmid && s->hist > 0) {
+            B200_CK(cudaMemcpy(s->fh[s->fpar].p, s->inbuf.p, (size_t)s->hist * s->in_es * sizeof(float), cudaMemcpyDeviceToDevice));
         }
     }
-    cudaDeviceSynchronize();      // the memsets above run on the legacy stream: finish them before the library's streams go on
+    B200_CK(cudaDeviceSynchronize());      // device-to-device copies on the legacy stream
+    return 0;
 }
 
 int Chain::add_xlator(double offsetHz, double samplerate) {
@@ -744,9 +778,12 @@ int Chain::add_deemph(double tau, double samplerate) {
 int Chain::add_af_chain(double afSR, double audioSR, bool highPass, double deemphTau) {
     int rc = add_resampler(afSR, audioSR);                                   // stereo_t == two packed floats: same kernels
     if (rc) { return rc; }
-    if (highPass && (rc = add_fir_c(highpass_taps(300.0, 100.0, audioSR), 1))) { return rc; }   // radio_module.h:597-598
+    if (highPass && (rc = add_af_highpass(audioSR))) { return rc; }
     if (deemphTau > 0.0 && (rc = add_deemph(deemphTau, audioSR))) { return rc; }
     return 0;
+}
+int Chain::add_af_highpass(double audioSR) {
+    return add_fir_c(highpass_taps(300.0, 100.0, audioSR), 1);              // radio_module.h:597-598
 }
 
 int Chain::add_noise_blanker(double rate, double level) {

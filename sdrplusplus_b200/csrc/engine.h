@@ -58,6 +58,7 @@ struct Stage {
     DevBuf fh[2];
     int fpar = 0;                // read fh[fpar], write fh[fpar ^ 1]
     bool fmid = false;
+    int role = 0;                // which radio block a front-end VFO built this stage for (api.cpp: VfoRole); 0 = none
     DevBuf taps_pm;              // taps in the fused kernel's phase-major order: row r = taps[q*D + r], pitch ceil(T/D)
     int pm_floats = 0;           // multiple of 4
     int upload_pm(const std::vector<float>& t, int rows_per_set, int sets);
@@ -101,6 +102,8 @@ struct FirCStage : Stage {
     FirCStage() { kind = K_FIRC; }
     int configure(const std::vector<float>& t, int decim_);
     int plan(int n) override;
+    // one output more than plan() can give: with decim 1 the stage is 1:1 (the radio's 300 Hz high-pass), and the front end keeps a
+    // VFO's bound the same when that filter is switched on or off (api.cpp: vfo_out_bound)
     int max_out(int n) const override { return (n + decim - 1) / decim + 1; }
     void reset_state() override { offset = 0; }
 };
@@ -141,6 +144,10 @@ struct SeqStage : Stage {
     int configure_ssb(int mode, double bandwidth, double samplerate, double attack, double decay);
     int configure_deemph(double tau, double samplerate);
     int configure_noise_blanker(double rate, double level);               // complex in, complex out
+    // the reference's coefficient setters: the device state (AGC amplitude, DC offset, de-emphasis output, blanker amplitude)
+    // is left alone, the next launch carries the new coefficient
+    void set_agc(double attack, double decay);                            // AGC::setAttack / setDecay (agc.h:32-44)
+    void set_deemph_tau(double tau, double samplerate);                   // Deemphasis::setTau (deephasis.h:31-36,91-94)
     int plan(int n) override { n_in = n; n_out = n; return n; }
     int max_out(int n) const override { return n; }
 };
@@ -231,6 +238,13 @@ struct Chain {
     int max_out(int n) const;
     int peek(int n) const;       // output count Chain::plan(n) would return, without moving any state (FIR-only chains; else -1)
     void reset_state();
+    // Blocks switched on or off between chunks (chain::setBlockEnabled): with the device idle the caller calls unfuse_history(),
+    // edits `st` in place (a 1:1 stage of the same sample size in or out; a stage that stays keeps its buffers), then
+    // restage().  A fused-middle stage keeps its history in fh[fpar], every other stage in front of its inbuf data:
+    // unfuse_history() copies the former into the latter for every stage, restage() rebuilds the fused plan and copies it back
+    // for the stages the new plan fuses.
+    int unfuse_history();
+    int restage();
     // builders (reference block -> stage list)
     int add_rxvfo(double inSR, double outSR, double bw, double offset);     // rx_vfo.h:17-31
     int add_xlator(double offsetHz, double samplerate);
@@ -246,12 +260,17 @@ struct Chain {
     int add_deemph(double tau, double samplerate);                          // filter::Deemphasis<stereo_t> (deephasis.h:14-28)
     // radio AF chain: RationalResampler<stereo_t> -> [300 Hz high-pass FIR] -> [Deemphasis]  (radio_module.h:99-110,546-553)
     int add_af_chain(double afSamplerate, double audioSamplerate, bool highPass, double deemphTau);
+    int add_af_highpass(double audioSamplerate);                            // taps::highPass(300, 100, audioSR) (radio_module.h:597-598)
     int add_wfm_rds(double deviationHz, double samplerate);                 // BroadcastFM's RDS branch: discriminator -> -57 kHz -> 5 kS/s (broadcast_fm.h:52-53,165-170)
     int add_noise_blanker(double rate, double level);                       // noise_reduction::NoiseBlanker (noise_blanker.h:12-17)
     int add_fmif(int bins);                                                 // noise_reduction::FMIF (fm_if.h:20-24)
     int add_squelch(double level);                                          // noise_reduction::PowerSquelch (power_squelch.h:16-20)
     int add_volume(double volume, bool muted);                              // dsp::audio::Volume (volume.h:13-17,39-42)
 };
+
+// block::reset of one stage: delay lines, fused history, mirrored counters and device state back to a fresh block's.  Memsets on
+// the legacy stream: the caller synchronises the device before the library's streams go on.
+void clear_stage_state(Stage& s);
 
 // Launch list of everything behind stage 1 of one chunk (parameter blocks by value).  Small chunks are launch-bound: the
 // list is hashed, and a chunk whose list was seen before replays a captured CUDA graph (one cudaGraphLaunch instead of

@@ -178,6 +178,13 @@ class FrontEnd:
     def set_vfo_bandwidth(self, vid, bw):
         L.check(self._l.b200_fe_set_vfo_bandwidth(self._h, vid, float(bw)))
 
+    def set_vfo_config(self, vid, cfg):
+        """The radio module's setters: the VFO takes `cfg` (a VfoConfig) at the next chunk, every block keeping its state
+        (b200_fe_set_vfo_config).  Raises on a change that needs a new demodulator; the VFO is then left as it was."""
+        c = cfg.to_c()
+        L.check(self._l.b200_fe_set_vfo_config(self._h, vid, C.byref(c)))
+        self.vfos[vid] = cfg
+
     def set_ingest_scale(self, fmt, scale):
         """Conversion factor of the next int16 / int8 chunks (a compressed-stream packet's scaler); <= 0: default."""
         L.check(self._l.b200_fe_set_ingest_scale(self._h, int(fmt), float(scale)))

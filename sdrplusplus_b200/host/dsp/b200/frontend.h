@@ -57,6 +57,10 @@ namespace dsp::b200 {
         }
         void setVFOOffset(int id, double offset) { b200_fe_set_vfo_offset(fe, id, offset); }
         void setVFOBandwidth(int id, double bandwidth) { b200_fe_set_vfo_bandwidth(fe, id, bandwidth); }
+        // the radio module's volume / squelch / blanker / noise-reduction / de-emphasis / AGC setters: taken at the next chunk,
+        // every block keeps its state, the worker keeps running (b200_fe_set_vfo_config); returns B200_EINVAL for a change
+        // that needs a new demodulator (removeVFO + addVFO)
+        int setVFOConfig(int id, const b200_vfo_cfg& cfg) { return b200_fe_set_vfo_config(fe, id, &cfg); }
         // IQFrontEnd::setDCBlocking / setInvertIQ (iq_frontend.cpp:117-123): take effect at the next chunk
         void setDCBlocking(bool enabled) { b200_fe_set_dc_blocking(fe, enabled); }
         void setInvertIQ(bool enabled) { b200_fe_set_invert_iq(fe, enabled); }

@@ -73,6 +73,7 @@ SIGNATURES = {
     "b200_fe_remove_vfo": (_i, [_vp, _i]),
     "b200_fe_set_vfo_offset": (_i, [_vp, _i, _d]),
     "b200_fe_set_vfo_bandwidth": (_i, [_vp, _i, _d]),
+    "b200_fe_set_vfo_config": (_i, [_vp, _i, C.POINTER(VfoCfg)]),
     "b200_fe_vfo_count": (_i, [_vp]),
     "b200_fe_vfo_max_out": (_i, [_vp, _i, _i]),
     "b200_fe_fft_max_lines": (_i, [_vp, _i]),
