@@ -123,13 +123,15 @@ static long double effective_omega(double rad) {
 }
 
 void XdStage::set_offset_rad(double rad) {
-    if (gpad.p && !retuned) { w_prev = w; retuned = true; }   // a retune of a running stage
     offset_rad = rad;
     long double turns = effective_omega(rad) / kTwoPiL;           // (-0.5, 0.5]
     long double scaled = turns * 18446744073709551616.0L;         // * 2^64
     if (scaled >= 9223372036854775807.0L) { scaled = 9223372036854775807.0L; }
     if (scaled <= -9223372036854775807.0L) { scaled = -9223372036854775807.0L; }
     w = (unsigned long long)(long long)llroundl(scaled);
+    // a retune after samples were translated with the current increment starts a segment; before that it replaces it
+    if (segs.empty() || segs.back().start < pos) { segs.push_back(Seg{ pos, phase, w }); }
+    else { segs.back().w = w; }
     taps_dirty = true;
 }
 
@@ -166,12 +168,29 @@ int XdStage::plan(int n) {
     n_in = n;
     chunk_offset = offset;
     chunk_phase0 = phase;
-    chunk_retuned = retuned && n > 0;
-    chunk_w_prev = w_prev;
-    if (n > 0) { retuned = false; }
     n_out = (offset < n) ? (n - offset + D - 1) / D : 0;
+    if (segs.empty()) { segs.push_back(Seg{ pos, phase, w }); }
+    // Every stage-1 build rotates the history with the current increment.  The outputs whose window starts before the
+    // newest boundary are recomputed by the edge kernel, which takes the history's phases from edge_tab.
+    // (the first segment is the stream start, not a boundary: before it lie no samples translated with another increment)
+    const long long b = segs.back().start - pos;                     // newest boundary, chunk-relative, <= 0
+    chunk_retuned = segs.size() > 1 && n_out > 0 && b > (long long)offset - (T - 1);
+    if (chunk_retuned) {
+        chunk_edge_start = (int)b;
+        edge_tab.resize((size_t)(T - 1));
+        size_t s = 0;
+        for (int j = 0; j < T - 1; j++) {
+            const long long a = pos + j - (T - 1);                   // absolute index of history sample j - (T-1)
+            while (s + 1 < segs.size() && segs[s + 1].start <= a) { s++; }
+            edge_tab[(size_t)j] = segs[s].phase + segs[s].w * (unsigned long long)(a - segs[s].start);
+        }
+    }
     offset = offset + n_out * D - n;
     phase += w * (unsigned long long)(long long)n;
+    pos += n;
+    size_t drop = 0;
+    while (drop + 1 < segs.size() && segs[drop + 1].start <= pos - (T - 1)) { drop++; }
+    if (drop) { segs.erase(segs.begin(), segs.begin() + (long)drop); }
     return n_out;
 }
 
@@ -1162,8 +1181,17 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
                 p.job[v].n_out = x->n_out;
                 p.job[v].T = x->T;
                 p.job[v].h = x->hdev.as<float>();
-                p.job[v].w_prev = x->chunk_w_prev;
                 p.job[v].retuned = x->chunk_retuned ? 1 : 0;
+                if (x->chunk_retuned) {
+                    const size_t bytes = x->edge_tab.size() * sizeof(unsigned long long);
+                    if (!x->edge_ph.p || x->edge_ph.bytes < bytes) {
+                        int rc = x->edge_ph.alloc((size_t)RAW_HIST * sizeof(unsigned long long));
+                        if (rc) { return rc; }
+                    }
+                    B200_CK(cudaMemcpyAsync(x->edge_ph.p, x->edge_tab.data(), bytes, cudaMemcpyHostToDevice, stream));
+                    p.job[v].hphase = x->edge_ph.as<unsigned long long>();
+                    p.job[v].edge_start = x->chunk_edge_start;
+                }
                 p.QP = std::max(p.QP, x->QP);
             }
             // slots: pair VFOs whose complex taps are exact conjugates (offsets +f / -f, same real prototype, same

@@ -76,8 +76,17 @@ struct XdStage : Stage {
     int D = 1, T = 1;
     std::vector<float> h;        // real taps of the first decimation stage ({1} for a pure translate)
     double offset_rad = 0.0;     // hzToRads(-vfoOffset, fs) as the reference passes it to the xlator
-    unsigned long long phase = 0, w = 0, w_prev = 0;
-    bool retuned = false, chunk_retuned = false; unsigned long long chunk_w_prev = 0;
+    unsigned long long phase = 0, w = 0;
+    long long pos = 0;           // input samples consumed since the stream (or the last reset) began
+    // Retunes still inside a tap window.  A sample keeps the rotation it was translated with: segment s covers the
+    // samples from segs[s].start up to the next segment's start, with phase(i) = segs[s].phase + segs[s].w * (i - start).
+    // The last segment is the current increment; a segment is dropped once T-1 samples lie past its successor's start.
+    struct Seg { long long start; unsigned long long phase, w; };
+    std::vector<Seg> segs;
+    bool chunk_retuned = false;  // this chunk has outputs whose window starts before the newest boundary
+    int chunk_edge_start = 0;    // newest boundary, chunk-relative (<= 0)
+    std::vector<unsigned long long> edge_tab;   // phase of chunk-relative samples -(T-1) .. -1 (when chunk_retuned)
+    DevBuf edge_ph;              // edge_tab on the device
     DevBuf hdev;                 // real taps on the device (retune edge kernel)
     int offset = 0;              // DecimatingFIR::offset
     DevBuf gpad;                 // complex taps, padded
@@ -90,7 +99,7 @@ struct XdStage : Stage {
     int upload_taps(cudaStream_t s);
     int plan(int n) override;
     int max_out(int n) const override { return (n + D - 1) / D + 1; }
-    void reset_state() override { phase = 0; offset = 0; retuned = false; }
+    void reset_state() override { phase = 0; offset = 0; pos = 0; segs.assign(1, Seg{ 0, 0, w }); chunk_retuned = false; }
     unsigned long long chunk_phase0 = 0; int chunk_offset = 0;   // snapshot used by this chunk's launch
 };
 

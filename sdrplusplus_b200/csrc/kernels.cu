@@ -144,8 +144,9 @@ __global__ void __launch_bounds__(128) k_xd_simple(const __grid_constant__ XdPar
 #include "rds.cuh"
 
 // ------------------------------------------------------------------------------------------------
-// retune edge: outputs whose tap window straddles the chunk start when the VFO offset changed at this
-// boundary.  Explicit per-sample rotation (old increment for history, new one for this chunk), real taps.
+// retune edge: outputs whose tap window starts before the newest retune boundary.  Explicit per-sample
+// rotation (each history sample with the phase it was translated with, this chunk's with the current increment),
+// real taps.
 // ------------------------------------------------------------------------------------------------
 template <int FMT>
 __global__ void __launch_bounds__(128) k_xd_edge(const __grid_constant__ XdParams p) {
@@ -155,12 +156,12 @@ __global__ void __launch_bounds__(128) k_xd_edge(const __grid_constant__ XdParam
     if (m >= J.n_out) { return; }
     const int T = J.T;
     const long long i0 = (long long)J.offset + (long long)m * p.D - (T - 1);
-    if (i0 >= 0) { return; }
+    if (i0 >= J.edge_start) { return; }
     float ar = 0.0f, ai = 0.0f;
     for (int k = 0; k < T; k++) {
         long long i = i0 + k;
         float2 x = load_x<FMT>(p, i);
-        unsigned long long ph = J.phase0 + ((i < 0) ? J.w_prev : J.w) * (unsigned long long)i;
+        unsigned long long ph = (i < 0) ? J.hphase[T - 1 + i] : J.phase0 + J.w * (unsigned long long)i;
         float2 z = cmulf(x, phasor_u64(ph));
         float t = __ldg(J.h + k);
         ar = fmaf(z.x, t, ar);
@@ -1046,7 +1047,7 @@ cudaError_t launch_xd_edge(const XdParams& p, int fmt, cudaStream_t s, int* nlau
     for (int v = 0; v < p.njobs; v++) {
         if (!p.job[v].retuned || p.job[v].n_out <= 0) { continue; }
         any = true;
-        int need = p.job[v].T - 1 - p.job[v].offset;          // outputs with i_m < 0
+        int need = p.job[v].edge_start + p.job[v].T - 1 - p.job[v].offset;   // outputs with i_m < edge_start
         int me = need > 0 ? (need + p.D - 1) / p.D : 0;
         if (me > p.job[v].n_out) { me = p.job[v].n_out; }
         if (me > medge) { medge = me; }

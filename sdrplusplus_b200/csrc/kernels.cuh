@@ -23,11 +23,12 @@ struct XdJob {
     int offset;             // DecimatingFIR::offset for this chunk (decimating_fir.h:50), 0 <= offset
     int n_out;              // outputs this chunk
     int T;                  // tap count
-    // retune at this chunk boundary (FrequencyXlator::setOffset keeps `phase`, frequency_xlator.h:25-29):
-    // history samples (index < 0) were rotated with w_prev, new samples with w.  The edge kernel recomputes
-    // the few outputs whose window straddles index 0 with the real taps h.
+    // retunes inside the tap window (FrequencyXlator::setOffset keeps `phase`, frequency_xlator.h:25-29): history
+    // sample i < 0 was rotated by hphase[T-1+i], samples from edge_start on by phase0 + w*i.  The edge kernel
+    // recomputes the outputs whose window starts before edge_start with the real taps h.
     const float* h;         // real taps (T)
-    unsigned long long w_prev;
+    const unsigned long long* hphase;   // T-1 phases (turns * 2^64) of the history samples
+    int edge_start;         // newest retune boundary, chunk-relative (<= 0)
     int retuned;
 };
 struct XdParams {

@@ -15,13 +15,11 @@ bound through sum_k |h_k|.  No tolerance here is fitted to a run.
 """
 import numpy as np
 import pytest
-from scipy.signal import oaconvolve
 
+from f64_ref import REF_FLOOR, U, _abs_parts, _corr, _gate_vfo, _hist, fir_f64
 from util import noise_iq, rel_rms
 
-U = 2.0 ** -24                      # unit round-off of fp32
-REF_FLOOR = 2.0 ** -40              # float64 FFT convolution error, relative to sum|h| max|x|: far below any fp32 rounding
-MAX_CHUNK = 1000000                 # a stand-alone block's chunk limit (STREAM_BUFFER_SIZE)
+MAX_CHUNK = 1000000                # a stand-alone block's chunk limit (STREAM_BUFFER_SIZE)
 
 # ---------------------------------------------------------------------------------------------- routing (mirrors engine.cpp)
 DFR_R = {(4, 27): 8, (2, 69): 4, (2, 12): 8, (8, 54): 4, (8, 44): 4, (8, 36): 4}   # outputs per thread (dfir_reg.cuh:107-112)
@@ -53,37 +51,7 @@ def routes_poly_reg(L, M, tpp):
 
 
 # ---------------------------------------------------------------------------------------------- float64 references
-def _corr(x, h):
-    """z[o] = sum_k h[k] x[o + k] for o = 0 .. len(x) - len(h)  (float64)"""
-    if x.size < h.size:
-        return np.zeros(0, x.dtype)
-    if h.size <= 64 or x.size <= 4 * h.size:
-        return np.convolve(x, h[::-1], "valid")
-    return oaconvolve(x, h[::-1], "valid")
-
-
-def _hist(v, k):
-    return np.concatenate([np.zeros(k, v.dtype), v])
-
-
-def _abs_parts(x):
-    return np.abs(x.real) + (np.abs(x.imag) if np.iscomplexobj(x) else 0.0)
-
-
-def fir_f64(x, e, h, D=1):
-    """FIR / DecimatingFIR from zero history: y[m] = sum_k h[k] xh[m D + k], xh = [T-1 zeros | x].
-    x: float64 input, e: per-sample bound of x's error (None = exact fp32 input).  Returns (y, bound of y)."""
-    h = np.asarray(h, np.float64)
-    T = h.size
-    y = _corr(_hist(x, T - 1), h)[::D]
-    a = _abs_parts(x) + (2.0 * e if e is not None else 0.0)
-    ah = np.abs(h)
-    b = (T + 2) * U * _corr(_hist(a, T - 1), ah)[::D]
-    if e is not None:
-        b = b + _corr(_hist(e, T - 1), ah)[::D]
-    return y, b + REF_FLOOR * ah.sum() * (float(a.max()) if a.size else 0.0)
-
-
+# (FIR / DecimatingFIR: f64_ref.fir_f64)
 def poly_bank(taps, L):
     """buildPolyphaseBank: bank[(L-1) - i % L][i // L] = taps[i], zero-padded to ceil(T / L) taps per phase"""
     taps = np.asarray(taps, np.float64)
@@ -530,7 +498,6 @@ SCHED_C = [0, 1, 7, 100003] + [240000] * 6 + [131071, 5, 0, 160001, 3, 120000, 2
 FS_G = 100e6
 OFFS_G = [5e6, -5e6, 15e6, -15e6, 25e6, -25e6, 35e6, -35e6]
 SCHED_G = [0, 1, 300001] + [1 << 20] * 3 + [7, 499999, 777777]
-EDGE = 64
 C_OPTIONS = [{}, {"tails": 1}, {"tails": 0}, {"ft_regall": 0}, {"ft_prereg": 0}]
 
 
@@ -592,24 +559,6 @@ def _oracle_raw(oracle, x, fs, sched, cfgs):
 def c_oracle(oracle, c_input):
     cfgs = [(o, r, 0.8 * r) for o, r in zip(_c_offsets(), C_RATES)]
     return cfgs, _oracle_raw(oracle, c_input, FS_C, SCHED_C, cfgs)
-
-
-def _gate_vfo(parts_gpu, parts_ref):
-    """count, rel_rms, fitted complex gain and edge-against-interior for one VFO"""
-    assert [p.size for p in parts_gpu] == [p.size for p in parts_ref]
-    y = np.concatenate(parts_gpu).astype(np.complex128)
-    yo = np.concatenate(parts_ref).astype(np.complex128)
-    e_rms = rel_rms(y, yo)
-    g = np.vdot(yo, y) / np.vdot(yo, yo)
-    e = np.abs(y - yo) / np.sqrt(np.mean(np.abs(yo) ** 2))
-    edge = np.zeros(y.size, bool)
-    for b in np.cumsum([0] + [p.size for p in parts_ref[:-1]]):
-        edge[max(0, b - EDGE): b + EDGE] = True
-    assert edge.any() and (~edge).sum() >= 1000
-    p999 = float(np.percentile(e[~edge], 99.9))
-    ratio = float(e[edge].max() / p999) if p999 > 0 else (0.0 if e[edge].max() == 0 else np.inf)
-    return {"rel_rms": e_rms, "gain_re": float(g.real), "gain_im": float(g.imag), "abs_g_minus_1": float(abs(g - 1)),
-            "edge_over_p999": ratio, "outputs": int(y.size)}
 
 
 def _check(res):
