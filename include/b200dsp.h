@@ -228,6 +228,26 @@ int b200_fe_set_vfo_bandwidth(b200_fe* fe, int id, double bandwidth);
  * on from it when switched on again (b200_fe_reset clears it).  demod, out_samplerate, deviation, low_pass and
  * af_samplerate need a new demodulator: B200_EINVAL (remove the VFO and add it again).  Output counts never change. */
 int b200_fe_set_vfo_config(b200_fe* fe, int id, const b200_vfo_cfg* cfg);
+/* IQFrontEnd::bindIQStream / unbindIQStream (core/src/signal_path/iq_frontend.h:34-35, iq_frontend.cpp:132-139): an IQ tap
+ * delivers the effective stream -- the chunk behind the pre-processing chain (decimator -> DC blocker -> conjugate), what the
+ * FFT branch and the VFOs read -- in one of the sample types below, interleaved I, Q.  Bytes per complex sample: CF32 8,
+ * U8 2, I8 2, I16 4, I32 8.  A tap takes an id of the VFO id space: its output travels in b200_outputs.vfo_out[id], vfo_cap[id]
+ * counts complex samples, vfo_count[id] is the number of samples of the effective stream in the chunk (the chunk's count,
+ * or what the decimator makes of it) and b200_fe_vfo_max_out(fe, id, count) returns `count`.  b200_fe_vfo_count counts taps.
+ * Bind and unbind follow the rules of add / remove VFO (b200_fe_set_decimation fails with B200_ESTATE after either); a tap id
+ * passed to the VFO setters or to b200_fe_remove_vfo, and a VFO id passed to b200_fe_unbind_iq, fail with B200_EINVAL.  A tap
+ * has no state of its own (b200_fe_reset resets the decimator and the DC blocker it reads from).  Every path that delivers
+ * VFO outputs delivers taps: b200_fe_process, submit / wait, B200_MEM_DEVICE outputs, b200_shard_*.
+ * Consumers' settings -- recorder (misc_modules/recorder, wav::Writer) WAV uint8 / int16 / int32 / float32: U8 / (I16, 32767) /
+ * (I32, 2147483647) / CF32; IQ exporter (misc_modules/iq_exporter) int8 / int16 / int32 / float32: (I8, 128) / (I16, 32768) /
+ * (I32, 2147483647) / CF32. */
+#define B200_IQ_CF32 0   /* complex_t: the stream bindIQStream hands out; scalar ignored                                  */
+#define B200_IQ_U8   1   /* wav.cpp uint8 rule: (unsigned char)(x * 127 + 128), truncated; scalar ignored                */
+#define B200_IQ_I8   2   /* rintf(clamp(x * scalar)) -- volk_32f_s32f_convert_8i / _16i / _32i; I32 saturates at INT_MAX */
+#define B200_IQ_I16  3   /*   exactly as b200_export_convert does                                                         */
+#define B200_IQ_I32  4
+int b200_fe_bind_iq(b200_fe* fe, int sample_type, float scalar);   /* returns an id */
+int b200_fe_unbind_iq(b200_fe* fe, int id);
 int b200_fe_vfo_count(b200_fe* fe);
 /* upper bound of output samples one chunk of `count` input samples can produce for VFO id */
 int b200_fe_vfo_max_out(b200_fe* fe, int id, int count);
@@ -271,7 +291,8 @@ long long b200_fe_stat(b200_fe* fe, const char* key);
  *            replays a captured CUDA graph (decimation offsets, resampler phases and buffer parities repeat after a few
  *            chunks of any fixed size); 0 = plain launches.  "tail_split" 2 = two independent branches (halves of the VFOs)
  *  "host_direct" -1 (default): VFO outputs in b200_host_alloc buffers are stored by the kernels themselves for chunks up to
- *            4 Mi samples (no copy to enqueue), 1 always, 0 never (copy engine)
+ *            4 Mi samples (no copy to enqueue), 1 always, 0 never (copy engine); IQ taps (b200_fe_bind_iq) under -1 only
+ *            when their output is at most 64 KiB, since the kernel's own stores over PCIe are slower than the copy engine
  *  "inflight" chunks between b200_fe_submit and b200_fe_wait: 2 (default) ... 4
  *  "s1_ctas" persistent CTAs of the TMA stage 1 (0 = one per SM)
  *  "pdl"     programmatic dependent launch for the chain kernels behind stage 1 (a successor is scheduled and loads its tables
@@ -287,7 +308,8 @@ int b200_fe_set_option(b200_fe* fe, const char* key, int value);
  * synchronises on the recorded events ("time_s1" must be on).  bench.py's roofline leg reads this. */
 int b200_fe_s1_stats(b200_fe* fe, double* ms_total, int* launches);
 /* the same for a launch group: 0 = stage 1, 1 = everything behind stage 1 of a chunk (register FIRs, fused tail, carries),
- * 2 = the spectrum branch of a chunk.  At most 512 samples per group are kept between two calls. */
+ * 2 = the spectrum branch of a chunk, 3 = the IQ taps of a chunk (k_iq_tap).  At most 512 samples per group are kept between
+ * two calls. */
 int b200_fe_group_stats(b200_fe* fe, int group, double* ms_total, int* launches);
 
 /* ------------------------------------------------------------------------------------------

@@ -254,7 +254,15 @@ struct VfoSlot {
     // B200_DEMOD_WFM_RDS_BITS: RDSDemod behind the chain, and where its records wait for the copy to a host buffer
     std::unique_ptr<RdsCore> rds;
     DevBuf rds_rec;
+    // an IQ tap (b200_fe_bind_iq) instead of a VFO: no chain, the chunk's effective stream in sample type tap_type (B200_IQ_*)
+    int tap_type = -1;
+    float tap_scalar = 0.0f;
 };
+static bool is_tap(const VfoSlot* v) { return v->tap_type >= 0; }
+// bytes per complex sample of an IQ tap's output (interleaved I, Q)
+static size_t iq_tap_bytes(int type) {
+    return type == B200_IQ_CF32 || type == B200_IQ_I32 ? 8 : (type == B200_IQ_I16 ? 4 : 2);
+}
 
 // input slots / event sets of a front end: a chunk uses slot (index % FE_SLOTS); up to FE_SLOTS chunks may be between submit and
 // wait (default two, option "inflight": small chunks over PCIe want the copy engine fed a few chunks ahead)
@@ -315,6 +323,12 @@ struct b200_fe {
     struct RdsPend { int id, n_in, bound; };
     std::vector<RdsPend> rds_pend[FE_SLOTS];
     b200_outputs* rds_out[FE_SLOTS] = {};    // whose vfo_count b200_fe_wait fills
+    // IQ taps (b200_fe_bind_iq): k_iq_tap runs on a stream of its own, forked behind the pre-processing like the spectrum
+    // branch and joined on join_stream; stream and events are made by the first bind
+    cudaStream_t tap_stream = nullptr;
+    cudaEvent_t ev_tap_go = nullptr, ev_tap_done = nullptr;
+    bool tap_read_pre = false;               // the taps of the last chunk read pre.out, which the next chunk's decimator rewrites
+    DevBuf tap_stage[FE_SLOTS];              // outputs that leave through a copy: one region per tap, 16-byte aligned
 };
 
 // (float)x * scale for the integer input formats: 1/32768 and 1/128 unless the caller set the scale of a
@@ -406,6 +420,9 @@ extern "C" void b200_fe_destroy(b200_fe* fe) {
     if (fe->own_stream) { cudaStreamDestroy(fe->own_stream); }
     if (fe->copy_stream) { cudaStreamDestroy(fe->copy_stream); }
     if (fe->fft_stream) { cudaStreamDestroy(fe->fft_stream); }
+    if (fe->tap_stream) { cudaStreamDestroy(fe->tap_stream); }
+    if (fe->ev_tap_go) { cudaEventDestroy(fe->ev_tap_go); }
+    if (fe->ev_tap_done) { cudaEventDestroy(fe->ev_tap_done); }
     if (fe->rds_count) { cudaFreeHost(fe->rds_count); }
     delete fe;
 }
@@ -573,9 +590,59 @@ extern "C" int b200_fe_add_vfo(b200_fe* fe, const b200_vfo_cfg* cfg) {
     return id;
 }
 
-static VfoSlot* get_vfo(b200_fe* fe, int id) {
+// a VFO or an IQ tap
+static VfoSlot* get_slot(b200_fe* fe, int id) {
     if (!fe || id < 0 || id >= (int)fe->vfos.size() || !fe->vfos[id]->used) { set_error("bad VFO id %d", id); return nullptr; }
     return fe->vfos[id].get();
+}
+static VfoSlot* get_vfo(b200_fe* fe, int id) {
+    VfoSlot* v = get_slot(fe, id);
+    if (v && is_tap(v)) { set_error("id %d is an IQ tap, not a VFO", id); return nullptr; }
+    return v;
+}
+
+// IQFrontEnd::bindIQStream / unbindIQStream (iq_frontend.h:34-35): an id of the VFO id space, no state of its own
+extern "C" int b200_fe_bind_iq(b200_fe* fe, int sample_type, float scalar) {
+    if (!fe) { set_error("null fe"); return B200_EINVAL; }
+    if (sample_type < B200_IQ_CF32 || sample_type > B200_IQ_I32) { set_error("bad IQ sample type %d", sample_type); return B200_EINVAL; }
+    if (!std::isfinite(scalar)) { set_error("IQ tap scalar must be finite"); return B200_EINVAL; }
+    std::lock_guard<std::mutex> lck(fe->mtx);
+    if (!fe->tap_stream) {
+        // the most urgent priority: the chunk's outputs wait for this short, memory-bound launch, which at the least urgent
+        // one queued behind stage 1 for up to 1.9 ms of a 3 ms step (DESIGN.md section 10)
+        int lo = 0, hi = 0;
+        cudaDeviceGetStreamPriorityRange(&lo, &hi);
+        if (cudaStreamCreateWithPriority(&fe->tap_stream, cudaStreamNonBlocking, hi) != cudaSuccess ||
+            cudaEventCreateWithFlags(&fe->ev_tap_go, cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&fe->ev_tap_done, cudaEventDisableTiming) != cudaSuccess) {
+            return cuda_fail(cudaGetLastError(), "IQ tap stream/event creation");
+        }
+    }
+    int id = -1;
+    for (size_t i = 0; i < fe->vfos.size(); i++) {
+        if (!fe->vfos[i]->used) { id = (int)i; break; }
+    }
+    if (id < 0) {
+        if (fe->vfos.size() >= B200_MAX_VFOS) { set_error("too many VFOs and IQ taps"); return B200_ECAP; }
+        fe->vfos.push_back(std::make_unique<VfoSlot>());
+        id = (int)fe->vfos.size() - 1;
+    }
+    else { fe->vfos[id] = std::make_unique<VfoSlot>(); }
+    VfoSlot* v = fe->vfos[id].get();
+    v->tap_type = sample_type;
+    v->tap_scalar = (sample_type == B200_IQ_CF32 || sample_type == B200_IQ_U8) ? 0.0f : scalar;
+    v->used = true;
+    return id;
+}
+extern "C" int b200_fe_unbind_iq(b200_fe* fe, int id) {
+    if (!fe) { set_error("null fe"); return B200_EINVAL; }
+    std::lock_guard<std::mutex> lck(fe->mtx);
+    VfoSlot* v = get_slot(fe, id);
+    if (!v) { return B200_EINVAL; }
+    if (!is_tap(v)) { set_error("id %d is a VFO, not an IQ tap", id); return B200_EINVAL; }
+    B200_CK(cudaDeviceSynchronize());
+    fe->vfos[id] = std::make_unique<VfoSlot>();
+    return 0;
 }
 
 extern "C" int b200_fe_remove_vfo(b200_fe* fe, int id) {
@@ -640,8 +707,9 @@ extern "C" int b200_fe_vfo_count(b200_fe* fe) {
     return n;
 }
 extern "C" int b200_fe_vfo_max_out(b200_fe* fe, int id, int count) {
-    VfoSlot* v = get_vfo(fe, id);
+    VfoSlot* v = get_slot(fe, id);
     if (!v) { return B200_EINVAL; }
+    if (is_tap(v)) { return std::max(count, 0); }      // one sample per sample of the effective stream
     return vfo_out_bound(v, count);
 }
 extern "C" int b200_fe_fft_max_lines(b200_fe* fe, int count) {
@@ -733,7 +801,7 @@ extern "C" int b200_fe_reset(b200_fe* fe) {
     std::lock_guard<std::mutex> lck(fe->mtx);
     B200_CK(cudaDeviceSynchronize());
     for (auto& v : fe->vfos) {
-        if (v->used) { v->chain.reset_state(); }
+        if (v->used && !is_tap(v.get())) { v->chain.reset_state(); }     // a tap has no state: it reads what the reset below clears
         if (v->used && v->rds) { int rcr = v->rds->reset(nullptr); if (rcr) { return rcr; } }
         for (auto& p : v->parked) { if (p) { clear_stage_state(*p); } }     // a block switched on later starts fresh
     }
@@ -896,7 +964,7 @@ static int apply_vfo_config(VfoSlot* v, const b200_vfo_cfg& n) {
 static int apply_pending(b200_fe* fe) {
     for (auto& up : fe->vfos) {
         VfoSlot* v = up.get();
-        if (!v->used) { continue; }
+        if (!v->used || is_tap(v)) { continue; }
         if (v->pend_cfg) {
             v->pend_cfg = false;
             int rc = apply_vfo_config(v, v->new_cfg);
@@ -1054,9 +1122,11 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
     const size_t in_bytes = (size_t)count * bytes_per_sample(in_fmt);
     // ---- capacity checks against the exact counts, before anything is enqueued and before any state moves ----
     std::vector<Chain*> chains;
-    std::vector<int> ids;
+    std::vector<int> ids, taps;
     for (size_t i = 0; i < fe->vfos.size(); i++) {
-        if (fe->vfos[i]->used) { chains.push_back(&fe->vfos[i]->chain); ids.push_back((int)i); }
+        if (!fe->vfos[i]->used) { continue; }
+        if (is_tap(fe->vfos[i].get())) { taps.push_back((int)i); }
+        else { chains.push_back(&fe->vfos[i]->chain); ids.push_back((int)i); }
     }
     // samples that reach the FFT branch and the VFOs: the chunk itself, or what the input decimator makes of it
     const int ecount = (fe->decim > 1) ? fe->pre.peek(count) : count;
@@ -1065,6 +1135,12 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
         int bound = vfo_out_bound(fe->vfos[ids[k]].get(), ecount);
         if (out->vfo_out[ids[k]] == nullptr || out->vfo_cap[ids[k]] < bound) {
             set_error("VFO %d output buffer too small: need room for %d samples (b200_fe_vfo_max_out)", ids[k], bound);
+            return B200_ECAP;
+        }
+    }
+    for (int id : taps) {
+        if (out->vfo_out[id] == nullptr || out->vfo_cap[id] < ecount) {
+            set_error("IQ tap %d output buffer too small: need room for %d samples (b200_fe_vfo_max_out)", id, ecount);
             return B200_ECAP;
         }
     }
@@ -1102,6 +1178,8 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
         const void* cur = dptr;
         int cur_fmt = in_fmt;
         if (fe->decim > 1) {
+            // the decimator's output is one buffer: the last chunk's IQ taps may still be reading it
+            if (fe->tap_read_pre) { B200_CK(cudaStreamWaitEvent(s, fe->ev_tap_done, 0)); }
             cudaError_t e = launch_convert_cf32(dptr, in_fmt, (float2*)fe->pre.st[0]->in_data(), count, fe_ingest_scale(fe, in_fmt), s);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
             fe->sch.launches++;
@@ -1158,6 +1236,51 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
     fe->lines_override = direct ? out->fft_out : nullptr;
     int nlines = 0;
     int rc;
+    // IQ taps: k_iq_tap reads the effective stream once and stores every tap, on its own stream so that neither the VFO
+    // branch nor the spectrum branch waits for it.  A tap writes the caller's buffer itself when that is device memory, or a
+    // b200_host_alloc buffer under the VFOs' rule -- with host_direct -1 only for outputs up to TAP_DIRECT_MAX bytes: the
+    // kernel's own stores over PCIe moved a 1 Mi-sample CF32 tap (8 MiB) at a third of the copy engine's rate.  Otherwise the
+    // tap fills its region of tap_stage[slot], copied out on the join stream.  tap_stage[slot] was last read by the copies of
+    // chunk nsub - FE_SLOTS, which b200_fe_wait has seen complete.
+    const size_t TAP_DIRECT_MAX = 64 << 10;
+    std::vector<size_t> tap_off(taps.size(), SIZE_MAX);
+    bool tap_forked = false;
+    if (!taps.empty() && count > 0) {
+        size_t need = 0, need_max = 0;
+        for (size_t k = 0; k < taps.size(); k++) {
+            const size_t b = iq_tap_bytes(fe->vfos[taps[k]]->tap_type);
+            const bool small = fe->host_direct > 0 || (size_t)count * b <= TAP_DIRECT_MAX;
+            if (direct || (host_direct && small && host_buffer_is_ours(out->vfo_out[taps[k]], (size_t)out->vfo_cap[taps[k]] * b))) { continue; }
+            tap_off[k] = need;
+            need += ((size_t)count * b + 15) & ~(size_t)15;
+            need_max += ((size_t)fe->max_eff * b + 15) & ~(size_t)15;
+        }
+        if (fe->tap_stage[slot].bytes < need && (rc = fe->tap_stage[slot].alloc(need_max, false))) { return rc; }
+        B200_CK(cudaEventRecord(fe->ev_tap_go, s));
+        B200_CK(cudaStreamWaitEvent(fe->tap_stream, fe->ev_tap_go, 0));
+        cudaEvent_t t_tap = fe->sch.timer_begin(3, fe->tap_stream);
+        IqTapParams tp;
+        memset(&tp, 0, sizeof(tp));
+        tp.in = dptr; tp.fmt = in_fmt; tp.n = count; tp.in_scale = fe_ingest_scale(fe, in_fmt);
+        auto aligned = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+        for (size_t k0 = 0; k0 < taps.size(); k0 += IQT_MAX) {
+            tp.njobs = 0;
+            tp.vec = aligned(dptr) ? 1 : 0;
+            for (size_t k = k0; k < taps.size() && k < k0 + IQT_MAX; k++) {
+                const VfoSlot* v = fe->vfos[taps[k]].get();
+                void* dst = tap_off[k] == SIZE_MAX ? out->vfo_out[taps[k]] : (void*)((char*)fe->tap_stage[slot].p + tap_off[k]);
+                tp.job[tp.njobs++] = IqTapJob{ dst, v->tap_type, v->tap_scalar };
+                tp.vec &= aligned(dst) ? 1 : 0;
+            }
+            cudaError_t e = launch_iq_tap(tp, fe->tap_stream);
+            if (e != cudaSuccess) { return cuda_fail(e, "launch_iq_tap"); }
+            fe->sch.launches++;
+        }
+        if (t_tap) { B200_CK(cudaEventRecord(t_tap, fe->tap_stream)); }
+        B200_CK(cudaEventRecord(fe->ev_tap_done, fe->tap_stream));
+        tap_forked = true;
+    }
+    fe->tap_read_pre = tap_forked && fe->decim > 1 && !fe->dc_block && !fe->invert_iq;
     // fork the spectrum branch first; its join (a wait on the main stream) comes after the VFO branch has been
     // enqueued, so the two overlap on the device
     const long long hp1 = host_clock_ns();
@@ -1203,6 +1326,7 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
         B200_CK(cudaStreamWaitEvent(os, fe->ev_fft_done, 0));
         fe->fft_join_pending = false;
     }
+    if (tap_forked) { B200_CK(cudaStreamWaitEvent(os, fe->ev_tap_done, 0)); }
     // the input chunk is no longer needed once stage 1, the raw carry (both in front of the tail on its stream) and the
     // spectrum branch are done
     B200_CK(cudaEventRecord(fe->ev_compute[slot], os));
@@ -1222,6 +1346,13 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
         out->vfo_count[ids[k]] = c->n_out;
         if (c->n_out > 0 && !vdirect[k]) {
             B200_CK(cudaMemcpyAsync(out->vfo_out[ids[k]], c->out.p, (size_t)c->n_out * c->out_es * sizeof(float), kind, os));
+        }
+    }
+    for (size_t k = 0; k < taps.size(); k++) {
+        out->vfo_count[taps[k]] = count;
+        if (count > 0 && tap_off[k] != SIZE_MAX) {
+            B200_CK(cudaMemcpyAsync(out->vfo_out[taps[k]], (const char*)fe->tap_stage[slot].p + tap_off[k],
+                                    (size_t)count * iq_tap_bytes(fe->vfos[taps[k]]->tap_type), kind, os));
         }
     }
     out->fft_lines = nlines;

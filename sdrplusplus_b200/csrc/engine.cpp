@@ -861,7 +861,7 @@ cudaEvent_t Scheduler::timer_begin(int group, cudaStream_t s) {
     return t1;
 }
 int Scheduler::group_stats(int group, double* ms_total, int* n) {
-    if (group < 0 || group > 2) { set_error("bad timer group"); return B200_EINVAL; }
+    if (group < 0 || group > 3) { set_error("bad timer group"); return B200_EINVAL; }
     Timer& t = timers[group];
     double tot = 0.0;
     for (size_t i = 0; i + 1 < t.used; i += 2) {

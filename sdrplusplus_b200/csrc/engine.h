@@ -330,11 +330,12 @@ struct Scheduler {
     bool pair_conjugates = true;   // stage 1: VFOs at +f / -f share their multiply-accumulates (exact identity)
     // optional device-side timing (bench.py's roofline legs): CUDA events around a launch group on the stream it runs on.
     // group 0 = stage 1 (stream), 1 = everything behind stage 1 of a chunk: register FIRs, fused tail, carries (tail stream),
-    // 2 = the spectrum branch of a chunk (its own stream; recorded by the front end).  At most TIMER_MAX samples per group.
+    // 2 = the spectrum branch of a chunk (its own stream; recorded by the front end), 3 = the IQ taps of a chunk (their own
+    // stream; recorded by the front end).  At most TIMER_MAX samples per group.
     bool time_s1 = false;
     static const size_t TIMER_MAX = 512;
     struct Timer { std::vector<cudaEvent_t> ev; size_t used = 0; };
-    Timer timers[3];
+    Timer timers[4];
     cudaEvent_t timer_begin(int group, cudaStream_t s);      // returns the stop event to record, nullptr when off / full
     int group_stats(int group, double* ms_total, int* launches);   // synchronises the recorded events, then clears them
     int s1_stats(double* ms_total, int* launches) { return group_stats(0, ms_total, launches); }

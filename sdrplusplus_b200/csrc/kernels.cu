@@ -660,6 +660,7 @@ __global__ void __launch_bounds__(512) k_fft_p2(const __grid_constant__ FftPlanD
 
 #include "fft_reg.cuh"
 #include "preproc.cuh"
+#include "iqtap.cuh"
 
 template <int FMT>
 __global__ void __launch_bounds__(256) k_convert(const void* __restrict__ src, float2* __restrict__ dst, int n, float sc) {
@@ -1346,30 +1347,23 @@ __global__ void __launch_bounds__(256) k_export(const float* __restrict__ in, lo
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) { return; }
     const float x = __ldg(in + i);
-    if (type == EXP_U8) {
-        // bufU8[i] = (samples[i] * 127.0f) + 128.0f   (float -> uint8_t conversion truncates)
-        const float v = __fadd_rn(__fmul_rn(x, 127.0f), 128.0f);
-        reinterpret_cast<unsigned char*>(out)[i] = (unsigned char)__float2int_rz(v);
-    }
-    else if (type == EXP_I8) {
-        float r = __fmul_rn(x, scalar);
-        r = fminf(fmaxf(r, -128.0f), 127.0f);
-        reinterpret_cast<signed char*>(out)[i] = (signed char)__float2int_rn(r);
-    }
-    else if (type == EXP_I16) {
-        float r = __fmul_rn(x, scalar);
-        r = fminf(fmaxf(r, -32768.0f), 32767.0f);
-        reinterpret_cast<short*>(out)[i] = (short)__float2int_rn(r);
-    }
-    else {
-        float r = __fmul_rn(x, scalar);
-        r = fminf(fmaxf(r, -2147483648.0f), 2147483648.0f);
-        reinterpret_cast<int*>(out)[i] = __float2int_rn(r);          // saturates at INT_MAX where the CPU conversion overflows
-    }
+    // the element rules are iqtap.cuh's, shared with the front end's IQ taps
+    if (type == EXP_U8) { reinterpret_cast<unsigned char*>(out)[i] = iq_rule_u8(x); }
+    else if (type == EXP_I8) { reinterpret_cast<signed char*>(out)[i] = iq_rule_i8(x, scalar); }
+    else if (type == EXP_I16) { reinterpret_cast<short*>(out)[i] = iq_rule_i16(x, scalar); }
+    else { reinterpret_cast<int*>(out)[i] = iq_rule_i32(x, scalar); }
 }
 cudaError_t launch_export(const float* in, long long n, int type, float scalar, void* out, cudaStream_t s) {
     if (n <= 0) { return cudaSuccess; }
     k_export<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(in, n, type, scalar, out);
+    return cudaGetLastError();
+}
+cudaError_t launch_iq_tap(const IqTapParams& p, cudaStream_t s) {
+    if (p.n <= 0 || p.njobs <= 0) { return cudaSuccess; }
+    const int grid = cdiv(cdiv(p.n, IQT_GROUP), IQT_THREADS);
+    if (p.fmt == FMT_CF32) { k_iq_tap<FMT_CF32><<<grid, IQT_THREADS, 0, s>>>(p); }
+    else if (p.fmt == FMT_CS16) { k_iq_tap<FMT_CS16><<<grid, IQT_THREADS, 0, s>>>(p); }
+    else { k_iq_tap<FMT_CS8><<<grid, IQT_THREADS, 0, s>>>(p); }
     return cudaGetLastError();
 }
 // first index of the maximum VALUE (not magnitude) of n floats: volk_32f_index_max_32u.  One CTA; key = (value, -index).

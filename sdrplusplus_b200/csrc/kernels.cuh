@@ -395,6 +395,20 @@ cudaError_t launch_preproc(const DcbParams& p, cudaStream_t s, int* nlaunch);
 cudaError_t launch_convert_cf32(const void* src, int fmt, float2* dst, int n, float scale, cudaStream_t s);
 enum { EXP_U8 = 0, EXP_I8 = 1, EXP_I16 = 2, EXP_I32 = 3 };
 cudaError_t launch_export(const float* in, long long n, int type, float scalar, void* out, cudaStream_t s);
+// ---- IQ taps (iqtap.cuh): the front end's effective stream in the recorder's / IQ exporter's sample types ----
+enum { IQT_CF32 = 0, IQT_U8 = 1, IQT_I8 = 2, IQT_I16 = 3, IQT_I32 = 4 };    // must match B200_IQ_* of include/b200dsp.h
+#define IQT_MAX 8
+struct IqTapJob { void* out; int type; float scalar; };
+struct IqTapParams {
+    const void* in;          // the effective stream of this chunk, format fmt
+    int fmt;
+    int n;                   // complex samples
+    float in_scale;          // integer formats: sample = (float)x * in_scale
+    int vec;                 // in and every job's out are 16-byte aligned
+    int njobs;
+    IqTapJob job[IQT_MAX];
+};
+cudaError_t launch_iq_tap(const IqTapParams& p, cudaStream_t s);
 cudaError_t launch_index_max(const float* in, long long n, float* out_val, cudaStream_t s);
 // start/len: per-pixel bin ranges built on the host with the reference's fp32 index loop
 cudaError_t launch_zoom_hold_tbl(const float* line, const int* start, const int* len, int out_size, float* out,

@@ -114,6 +114,13 @@ def rds_symbols(buf, n):
     return r["soft"].copy(), r["bit"].astype(np.uint8)
 
 
+def iq_tap_array(sample_type, n):
+    """An empty output of an IQ tap: complex64 for IQ_CF32, (n, 2) interleaved I, Q integers for the other types."""
+    if sample_type == L.IQ_CF32:
+        return np.empty(n, np.complex64)
+    return np.empty((n, 2), {L.IQ_U8: np.uint8, L.IQ_I8: np.int8, L.IQ_I16: np.int16, L.IQ_I32: np.int32}[sample_type])
+
+
 def _as_input(iq, fmt):
     dt, per = _NP_FMT[fmt]
     a = np.ascontiguousarray(iq, dtype=dt).reshape(-1)
@@ -132,6 +139,7 @@ class FrontEnd:
         self.max_chunk = int(max_chunk)
         self.fft_size = 0
         self.vfos = {}
+        self.taps = {}               # IQ tap id -> sample type
 
     def close(self):
         if getattr(self, "_h", None):
@@ -171,6 +179,17 @@ class FrontEnd:
     def remove_vfo(self, vid):
         L.check(self._l.b200_fe_remove_vfo(self._h, vid))
         self.vfos.pop(vid, None)
+
+    def bind_iq(self, sample_type, scalar=0.0):
+        """IQFrontEnd::bindIQStream: the effective stream (behind decimation, DC blocking and conjugate) in one of the
+        IQ_* sample types, delivered by every later process() under the returned id (b200_fe_bind_iq)."""
+        tid = L.check(self._l.b200_fe_bind_iq(self._h, int(sample_type), float(scalar)))
+        self.taps[tid] = int(sample_type)
+        return tid
+
+    def unbind_iq(self, tid):
+        L.check(self._l.b200_fe_unbind_iq(self._h, tid))
+        self.taps.pop(tid, None)
 
     def set_vfo_offset(self, vid, offset):
         L.check(self._l.b200_fe_set_vfo_offset(self._h, vid, float(offset)))
@@ -227,6 +246,12 @@ class FrontEnd:
             bufs[vid] = b
             o.vfo_out[vid] = b.ctypes.data
             o.vfo_cap[vid] = cap
+        for tid, t in self.taps.items():
+            cap = self.vfo_max_out(tid, count)
+            b = iq_tap_array(t, max(cap, 1))
+            bufs[tid] = b
+            o.vfo_out[tid] = b.ctypes.data
+            o.vfo_cap[tid] = cap
         fft = None
         if self.fft_size:
             nl = self.fft_max_lines(count)
@@ -238,7 +263,7 @@ class FrontEnd:
 
     def process(self, iq, fmt=L.FMT_CF32):
         """Host numpy in, host numpy out.  Returns ({vfo_id: array}, fft_lines[n, N]); a DEMOD_WFM_RDS_BITS VFO gives the
-        pair (soft float32, bit uint8)."""
+        pair (soft float32, bit uint8), an IQ tap complex64 (IQ_CF32) or (n, 2) uint8 / int8 / int16 / int32."""
         a, count = _as_input(iq, fmt)
         o, bufs, fft = self._alloc_outputs(count)
         L.check(self._l.b200_fe_process(self._h, a.ctypes.data, count, fmt, L.MEM_HOST, C.byref(o)))
@@ -250,13 +275,15 @@ class FrontEnd:
                 continue
             y = bufs[vid][: 2 * n].copy()
             outs[vid] = y.view(np.complex64) if cfg.demod in (L.DEMOD_RAW, L.DEMOD_WFM_RDS) else y.reshape(-1, 2)
+        for tid in self.taps:
+            outs[tid] = bufs[tid][: o.vfo_count[tid]].copy()
         lines = fft[: o.fft_lines].copy() if fft is not None else np.empty((0, 0), np.float32)
         return outs, lines
 
     def process_chunks(self, iq, chunk, fmt=L.FMT_CF32):
         a, count = _as_input(iq, fmt)
         per = _NP_FMT[fmt][1]
-        acc = {vid: [] for vid in self.vfos}
+        acc = {vid: [] for vid in list(self.vfos) + list(self.taps)}
         lines = []
         for i in range(0, count, chunk):
             outs, ln = self.process(a[i * per:(i + chunk) * per], fmt)
@@ -266,7 +293,9 @@ class FrontEnd:
                 lines.append(ln)
         res = {}
         for vid, v in acc.items():
-            if self.vfos[vid].demod == L.DEMOD_WFM_RDS_BITS:
+            if vid in self.taps:
+                res[vid] = np.concatenate(v) if v else iq_tap_array(self.taps[vid], 0)
+            elif self.vfos[vid].demod == L.DEMOD_WFM_RDS_BITS:
                 res[vid] = (np.concatenate([p[0] for p in v]) if v else np.empty(0, np.float32),
                             np.concatenate([p[1] for p in v]) if v else np.empty(0, np.uint8))
             else:

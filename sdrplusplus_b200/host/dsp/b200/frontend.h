@@ -55,6 +55,31 @@ namespace dsp::b200 {
             }
             tempStart();
         }
+        // IQFrontEnd::bindIQStream / unbindIQStream (iq_frontend.h:34-35): the effective stream (behind the decimation and DC
+        // blocking given to init, and setInvertIQ) goes to every bound stream, whose buffer must hold a whole input chunk;
+        // each is a CF32 tap of the front end (b200_fe_bind_iq).  Any number of streams, up to the VFO id space.
+        void bindIQStream(stream<complex_t>* s) {
+            std::lock_guard<std::recursive_mutex> lk(ctrlMtx);
+            tempStop();
+            int id = b200_fe_bind_iq(fe, B200_IQ_CF32, 0.0f);
+            if (id >= 0) {
+                iqs_.push_back({ s, id });
+                registerOutput(s);
+            }
+            tempStart();
+        }
+        void unbindIQStream(stream<complex_t>* s) {
+            std::lock_guard<std::recursive_mutex> lk(ctrlMtx);
+            tempStop();
+            for (size_t i = 0; i < iqs_.size(); i++) {
+                if (iqs_[i].s != s) { continue; }
+                b200_fe_unbind_iq(fe, iqs_[i].id);
+                unregisterOutput(s);
+                iqs_.erase(iqs_.begin() + i);
+                break;
+            }
+            tempStart();
+        }
         void setVFOOffset(int id, double offset) { b200_fe_set_vfo_offset(fe, id, offset); }
         void setVFOBandwidth(int id, double bandwidth) { b200_fe_set_vfo_bandwidth(fe, id, bandwidth); }
         // the radio module's volume / squelch / blanker / noise-reduction / de-emphasis / AGC setters: taken at the next chunk,
@@ -84,6 +109,10 @@ namespace dsp::b200 {
                 o.vfo_out[i] = outs_[i]->writeBuf;
                 o.vfo_cap[i] = outs_[i]->bufferSize();
             }
+            for (auto& t : iqs_) {
+                o.vfo_out[t.id] = t.s->writeBuf;
+                o.vfo_cap[t.id] = t.s->bufferSize();
+            }
             o.fft_out = lines;
             o.fft_cap_lines = b200_fe_fft_max_lines(fe, count);
             o.out_mem = B200_MEM_HOST;
@@ -97,6 +126,10 @@ namespace dsp::b200 {
             }
             for (size_t i = 0; i < outs_.size(); i++) {
                 if (outs_[i] && o.vfo_count[i] > 0 && !outs_[i]->swap(o.vfo_count[i])) { return -1; }
+            }
+            // every bound stream gets every chunk, as IQFrontEnd's splitter hands it out (splitter.h:46-61)
+            for (auto& t : iqs_) {
+                if (!t.s->swap(o.vfo_count[t.id])) { return -1; }
             }
             return count;
         }
@@ -114,6 +147,8 @@ namespace dsp::b200 {
         stream<complex_t>* _in = nullptr;
         b200_fe* fe = nullptr;
         std::vector<stream<stereo_t>*> outs_;
+        struct BoundIQ { stream<complex_t>* s; int id; };
+        std::vector<BoundIQ> iqs_;
         float* lines = nullptr;
         int size = 0;
         float* (*acquire)(void*) = nullptr;

@@ -2,6 +2,7 @@
 // a stream, RxVFO -> BroadcastFM run as worker-thread blocks, the main thread reads stereo audio.  Prints one line
 // "<samples_out> <checksum>"; tests/test_host_adapter.py compares it with the oracle on the same seeded input.
 #include <cmath>
+#include <condition_variable>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -10,6 +11,7 @@
 #include "dsp/channel/rx_vfo.h"
 #include "dsp/demod/broadcast_fm.h"
 #include "dsp/b200/frontend.h"
+#include "dsp/sink/handler_sink.h"
 #include "radio/rds_demod.h"
 #include "dsp/compression/sample_stream_compressor.h"   // compiled here; exercised through the C ABI in tests/test_gpu_parity.py
 
@@ -62,6 +64,41 @@ int main(int argc, char** argv) {
         fwrite(audio.data(), sizeof(dsp::stereo_t), audio.size(), o);
         fclose(o);
         printf("%zu %d\n", audio.size(), g_lines);
+        return 0;
+    }
+    if (argc > 3 && !strcmp(argv[3], "iqtap")) {
+        // a baseband recorder's wiring: a sink::Handler<complex_t> worker on a stream bound with bindIQStream behind a
+        // front end that decimates by 4 and blocks DC (IQFrontEnd::init's decimRatio / dcBlocking); no FFT, no VFO
+        dsp::b200::FrontEnd fe;
+        fe.init(&input, fs, 0, 20.0, B200_WIN_NUTTALL, nullptr, nullptr, nullptr, 4, true);
+        dsp::stream<dsp::complex_t> iqs(chunk);
+        fe.bindIQStream(&iqs);
+        struct Rec { std::vector<dsp::complex_t> x; std::mutex m; std::condition_variable cv; size_t chunks = 0; } rec;
+        dsp::sink::Handler<dsp::complex_t> sink(&iqs, [](dsp::complex_t* d, int n, void* ctx) {
+            Rec* r = (Rec*)ctx;
+            std::lock_guard<std::mutex> lk(r->m);
+            r->x.insert(r->x.end(), d, d + n);
+            r->chunks++;
+            r->cv.notify_all();
+        }, &rec);
+        sink.start();
+        fe.start();
+        const size_t nch = iq.size() / chunk;
+        for (size_t i = 0; i < nch; i++) {
+            memcpy(input.writeBuf, &iq[i * chunk], chunk * sizeof(dsp::complex_t));
+            if (!input.swap(chunk)) { return 4; }
+        }
+        {
+            std::unique_lock<std::mutex> lk(rec.m);
+            rec.cv.wait(lk, [&] { return rec.chunks == nch; });
+        }
+        fe.stop();
+        sink.stop();
+        fe.unbindIQStream(&iqs);
+        FILE* o = fopen(argv[2], "wb");
+        fwrite(rec.x.data(), sizeof(dsp::complex_t), rec.x.size(), o);
+        fclose(o);
+        printf("%zu %zu\n", rec.x.size(), rec.chunks);
         return 0;
     }
     if (argc > 3 && !strcmp(argv[3], "rds")) {

@@ -14,6 +14,7 @@ WIN_RECTANGULAR, WIN_BLACKMAN, WIN_NUTTALL = 0, 1, 2
 DEMOD_RAW, DEMOD_WFM, DEMOD_NFM, DEMOD_AM, DEMOD_USB, DEMOD_LSB, DEMOD_DSB, DEMOD_WFM_STEREO, DEMOD_WFM_RDS = range(9)
 DEMOD_WFM_RDS_BITS = 9
 AGC_CARRIER, AGC_AUDIO = 0, 1
+IQ_CF32, IQ_U8, IQ_I8, IQ_I16, IQ_I32 = range(5)        # b200_fe_bind_iq sample types
 E = {0: "OK", -1: "EINVAL", -2: "ENODEV", -3: "ECUDA", -4: "ENOMEM", -5: "ECAP", -6: "ENOPLAN", -7: "ESTATE"}
 
 
@@ -74,6 +75,8 @@ SIGNATURES = {
     "b200_fe_set_vfo_offset": (_i, [_vp, _i, _d]),
     "b200_fe_set_vfo_bandwidth": (_i, [_vp, _i, _d]),
     "b200_fe_set_vfo_config": (_i, [_vp, _i, C.POINTER(VfoCfg)]),
+    "b200_fe_bind_iq": (_i, [_vp, _i, C.c_float]),
+    "b200_fe_unbind_iq": (_i, [_vp, _i]),
     "b200_fe_vfo_count": (_i, [_vp]),
     "b200_fe_vfo_max_out": (_i, [_vp, _i, _i]),
     "b200_fe_fft_max_lines": (_i, [_vp, _i]),
