@@ -1317,12 +1317,30 @@ static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const FftFrames& fr, flo
     return cudaGetLastError();
 }
 
+// gridDim.y holds a batch's frame index, so a batch of more frames is launched in slices of at most this many
+#define FFT_MAX_GRID_Y 65535
 cudaError_t launch_fft_frames(const FftPlanDev& pl, const FftFrames& fr, int fmt, float2* work, float* out_db,
                               float2* out_raw, cudaStream_t s, int* nlaunch, bool tables) {
-    if (fr.nbatch <= 0) { return cudaSuccess; }
-    if (fmt == FMT_CF32) { return launch_fft_fmt<FMT_CF32>(pl, fr, work, out_db, out_raw, s, nlaunch, tables); }
-    if (fmt == FMT_CS16) { return launch_fft_fmt<FMT_CS16>(pl, fr, work, out_db, out_raw, s, nlaunch, tables); }
-    return launch_fft_fmt<FMT_CS8>(pl, fr, work, out_db, out_raw, s, nlaunch, tables);
+    const int bps = fmt == FMT_CF32 ? 8 : (fmt == FMT_CS16 ? 4 : 2);
+    for (int f0 = 0; f0 < fr.nbatch; f0 += FFT_MAX_GRID_Y) {
+        // slice 0 keeps the staged part of its first frame; a later slice's first frame lies wholly in the chunk
+        FftFrames sl = fr;
+        sl.nbatch = std::min(fr.nbatch - f0, FFT_MAX_GRID_Y);
+        if (f0 > 0) {
+            sl.chunk = reinterpret_cast<const char*>(fr.chunk) + ((long long)f0 * fr.stride - fr.split) * bps;
+            sl.pre = nullptr;
+            sl.split = 0;
+        }
+        float2* const w = work + (size_t)f0 * pl.N;
+        float* const db = out_db ? out_db + (size_t)f0 * pl.N : nullptr;
+        float2* const raw = out_raw ? out_raw + (size_t)f0 * pl.N : nullptr;
+        cudaError_t e;
+        if (fmt == FMT_CF32) { e = launch_fft_fmt<FMT_CF32>(pl, sl, w, db, raw, s, nlaunch, tables); }
+        else if (fmt == FMT_CS16) { e = launch_fft_fmt<FMT_CS16>(pl, sl, w, db, raw, s, nlaunch, tables); }
+        else { e = launch_fft_fmt<FMT_CS8>(pl, sl, w, db, raw, s, nlaunch, tables); }
+        if (e != cudaSuccess) { return e; }
+    }
+    return cudaSuccess;
 }
 cudaError_t launch_fft_frame(const FftPlanDev& pl, const void* src, int fmt, float2* work, float* out_db,
                              float2* out_raw, cudaStream_t s, int* nlaunch) {
