@@ -269,7 +269,8 @@ long long b200_fe_launch_count(b200_fe* fe);
 /* counters by name: "launches", "chunks", "s1_tma_launches" (stage-1 launches of this process that ran the TMA-fed
  * filter-bank kernel), "graphs" / "graph_hits" / "graph_misses" (launch lists captured / replayed / launched plainly),
  * "host_ns_plan" / "host_ns_fft" / "host_ns_run" / "host_ns_join" / "host_ns_stage1" / "host_ns_tail" (host time spent inside
- * b200_fe_submit since creation, by section, in ns); -1 for an unknown key */
+ * b200_fe_submit since creation, by section, in ns), "fused_chains" (VFOs whose stages behind stage 1 are planned into one
+ * k_tail_fused launch per chunk); -1 for an unknown key */
 long long b200_fe_stat(b200_fe* fe, const char* key);
 /* Tuning / A-B switches (defaults are the fast paths; every variant is held to the same parity tests):
  *  "s1"      stage-1 kernel: 8 (default) filter-bank form fed by the TMA engine (cf32 chunks, VFO offsets on a common

@@ -733,6 +733,11 @@ extern "C" long long b200_fe_stat(b200_fe* fe, const char* key) {
     if (!strcmp(key, "graphs")) { return (long long)fe->sch.graphs.size(); }
     if (!strcmp(key, "host_ns_stage1")) { return fe->sch.host_ns[0]; }
     if (!strcmp(key, "host_ns_tail")) { return fe->sch.host_ns[1]; }
+    if (!strcmp(key, "fused_chains")) {
+        long long n = 0;
+        for (auto& v : fe->vfos) { n += (v->used && v->chain.fp.active) ? 1 : 0; }
+        return n;
+    }
     return -1;
 }
 extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {

@@ -16,23 +16,13 @@ bound through sum_k |h_k|.  No tolerance here is fitted to a run.
 import numpy as np
 import pytest
 
-from f64_ref import REF_FLOOR, U, _abs_parts, _corr, _gate_vfo, _hist, fir_f64
+from f64_ref import (DFR_R, MAX_CHUNK, POLY_REG, TS_TILE, _gate_vfo, cascade_counts, fir_counts, fir_f64, poly_bank, poly_f64,
+                     poly_out_index, routes_dfir_reg, schedule)
 from util import noise_iq, rel_rms
 
-MAX_CHUNK = 1000000                # a stand-alone block's chunk limit (STREAM_BUFFER_SIZE)
-
 # ---------------------------------------------------------------------------------------------- routing (mirrors engine.cpp)
-DFR_R = {(4, 27): 8, (2, 69): 4, (2, 12): 8, (8, 54): 4, (8, 44): 4, (8, 36): 4}   # outputs per thread (dfir_reg.cuh:107-112)
-DFR_MAXT = 72                                                                     # kernels.cuh: DfrParams.taps
-POLY_REG = {(16, 25), (5, 6), (2, 3), (4, 5), (2, 5)}                             # tails_reg.cuh:138-140
-TS_TILE = 256                                                                     # k_fir_reg / k_firr_reg outputs per CTA
 PR_PER = 32                                                                       # k_poly_reg periods per CTA
 PLAN_RATIO = {(2, 69): 2, (2, 12): 4, (4, 27): 8, (8, 54): 16, (8, 44): 32, (8, 36): 64}   # plan whose stage 0 is (D, T)
-
-
-def routes_dfir_reg(D, T):
-    """engine.cpp:1273-1277 (dfr_ok) with dfir_reg.cuh:100-102"""
-    return D > 1 and T <= DFR_MAXT and (D, T) in DFR_R
 
 
 def routes_fir_reg(D, T):
@@ -50,95 +40,8 @@ def routes_poly_reg(L, M, tpp):
     return (L, M) in POLY_REG and tpp <= 512
 
 
-# ---------------------------------------------------------------------------------------------- float64 references
-# (FIR / DecimatingFIR: f64_ref.fir_f64)
-def poly_bank(taps, L):
-    """buildPolyphaseBank: bank[(L-1) - i % L][i // L] = taps[i], zero-padded to ceil(T / L) taps per phase"""
-    taps = np.asarray(taps, np.float64)
-    tpp = -(-taps.size // L)
-    bank = np.zeros((L, tpp))
-    i = np.arange(taps.size)
-    bank[(L - 1) - i % L, i // L] = taps
-    return bank
-
-
-def poly_out_index(n, L, M):
-    """outputs m of an n-sample stream: off = m M // L (< n), bank row ph = m M % L"""
-    m = np.arange((n * L + M - 1) // M, dtype=np.int64)
-    return (m * M) // L, (m * M) % L
-
-
-def poly_f64(x, e, taps, L, M):
-    """PolyphaseResampler from zero history: y[m] = sum_j bank[ph][j] xh[off + j], xh = [tpp-1 zeros | x]"""
-    bank = poly_bank(taps, L)
-    tpp = bank.shape[1]
-    off, ph = poly_out_index(x.size, L, M)
-    xh = _hist(x, tpp - 1)
-    a = _abs_parts(x) + (2.0 * e if e is not None else 0.0)
-    ah = _hist(a, tpp - 1)
-    eh = _hist(e, tpp - 1) if e is not None else None
-    y = np.zeros(off.size, x.dtype)
-    b = np.zeros(off.size)
-    for p in range(L):
-        sel = ph == p
-        if not sel.any():
-            continue
-        o = off[sel]
-        y[sel] = _corr(xh, bank[p])[o]
-        b[sel] = (tpp + 2) * U * _corr(ah, np.abs(bank[p]))[o]
-        if eh is not None:
-            b[sel] += _corr(eh, np.abs(bank[p]))[o]
-    return y, b + REF_FLOOR * np.abs(bank).sum(axis=1).max() * (float(a.max()) if a.size else 0.0)
-
-
 # ---------------------------------------------------------------------------------------------- chunk bookkeeping
-def fir_counts(sched, D):
-    """per-chunk outputs and the chunk's offset into [history | data] (DecimatingFIR::process's `offset`)"""
-    off, outs, offs = 0, [], []
-    for n in sched:
-        no = (n - off + D - 1) // D if off < n else 0
-        offs.append(off)
-        outs.append(no)
-        off = off + no * D - n
-    return outs, offs
-
-
-def poly_counts(sched, L, M):
-    off, ph, outs = 0, 0, []
-    for n in sched:
-        avail = (n - off) * L - ph
-        no = (avail + M - 1) // M if avail > 0 else 0
-        tend = ph + no * M
-        off, ph = off + tend // L - n, tend % L
-        outs.append(no)
-    return outs
-
-
-def cascade_counts(sched, stages):
-    """stages: ("fir", D) / ("poly", L, M); returns the last stage's outputs per chunk"""
-    cur = list(sched)
-    for s in stages:
-        cur = fir_counts(cur, s[1])[0] if s[0] == "fir" else poly_counts(cur, s[1], s[2])
-    return cur
-
-
-def schedule(tile_in, T, total=200000, seed=0, repeat=None):
-    """0- and 1-sample chunks, one shorter than T-1, one CTA tile and one sample either side, a long chunk followed by short
-    ones (stale samples of the long one lie past the end of the short ones), >= 3 repeats of one size (the recorded launch
-    list is replayed as a graph), odd sizes (both parities of a decimation offset) filling up to `total`."""
-    rng = np.random.default_rng(seed)
-    rep = repeat or tile_in
-    s = [0, 1, max(0, (T - 2) // 2), 3, tile_in, tile_in + 1, tile_in - 1, 0, 1]
-    s += [min(MAX_CHUNK, max(60000, 8 * tile_in)), 7, 2, 13, 1]
-    s += [rep] * 6
-    while sum(s) + 12000 + tile_in + 1 < total:
-        s.append(int(rng.integers(500, 12000)) | 1)
-    s.append(tile_in + 1)
-    while sum(s) < total:
-        s.append(min(total - sum(s), MAX_CHUNK))
-    return [int(v) for v in s]
-
-
+# (the float64 references and schedule(): f64_ref)
 def predec_schedule(tile, T, seed):
     """behind a large predecimator a resampler tile is longer than a chunk: the same kinds of chunk, capped at the chunk
     limit, repeats of a whole resampler period, 6 M samples (~300 outputs at 1 kS/s from 20.48 MS/s)"""

@@ -37,14 +37,13 @@ import math
 import numpy as np
 import pytest
 
-from f64_ref import REF_FLOOR, U, _corr, _hist, fir_f64
+from f64_ref import (PFB_CASES, TWO64, _corr, _hist, _signed, drift_weights, fir_f64, pfb_detect, pfb_eps, plan_of,
+                     rotate_f64, stage1_f64, w_u64)
 from util import noise_iq
 
-TWO64 = 1 << 64
 FS = 100e6
 RAW_HIST = 1024                                       # engine.h: Scheduler::RAW_HIST
 XT_CASES = {(5, 5), (6, 5), (6, 6), (6, 7)}           # kernels.cu: XT_CASE (log2 D, QC)
-PFB_CASES = {(5, 5), (6, 5), (4, 5), (3, 7), (2, 7)}  # kernels.cu: PFB_CASE (log2 D, QC)
 XT_MAXTAPS = 512                                      # xd_tma.cuh
 CF32, CS16, CS8 = 0, 1, 2
 PS10M = [5e6, -5e6, 15e6, -15e6, 25e6, -25e6, 35e6, -35e6]     # PS 10, sigma -1 at 100 MS/s
@@ -53,54 +52,9 @@ PS8P = [12.5e6, -12.5e6, 37.5e6, -25e6]                         # PS 8, sigma +1
 PS8M = [6.25e6, -6.25e6, 18.75e6, -31.25e6]                     # PS 8, sigma -1
 OFFGRID = [5e6 + 1234.5, -7.3e6, 21e6 + 77.0]
 LIMIT_BASE = 25e6                                               # on this grid point the fp32 phasor steps come closest to the limit
-_KTWOPI = np.longdouble("6.283185307179586476925286766559")
 
 
 # ---------------------------------------------------------------------------------------------- mirrors of the host code
-def w_u64(offset_hz, fs):
-    """XdStage::set_offset_rad(hz_to_rads(-offset, fs)): angle of the fp32-rounded phasor, in turns * 2^64"""
-    rad = 2.0 * math.pi * (-offset_hz / fs)
-    dre, dim = np.float32(math.cos(rad)), np.float32(math.sin(rad))
-    turns = np.arctan2(np.longdouble(dim), np.longdouble(dre)) / _KTWOPI
-    scaled = turns * np.longdouble(18446744073709551616.0)
-    lim = np.longdouble(9223372036854775807.0)
-    scaled = min(max(scaled, -lim), lim)
-    return int(np.round(scaled)) % TWO64
-
-
-def _signed(r):
-    r %= TWO64
-    return r - TWO64 if r >= (1 << 63) else r
-
-
-def pfb_detect(ws, T):
-    """Scheduler::run: smallest P <= 10 with e^{j w P} within 8e-6 rad over the window of the same sign +-1 for every job,
-    mapped to the kernel's PS = 8 / 10 instantiation.  Returns (PS, sigma), (0, 1) when no filter-bank form applies."""
-    for P in range(1, 11):
-        tol = (8e-6 / 6.283185307179586) * P / T * 18446744073709551616.0
-        sg, ok = 0, True
-        for w in ws:
-            r = (w * P) % TWO64
-            d0, d1 = float(_signed(r)), float(_signed(r - (1 << 63)))
-            sv = 1 if abs(d0) <= tol else (-1 if abs(d1) <= tol else 0)
-            if sv == 0 or (sg != 0 and sv != sg):
-                ok = False
-                break
-            sg = sv
-        if not ok:
-            continue
-        for PS in (8, 10):
-            if PS % P == 0:
-                return PS, (-1 if (sg < 0 and (PS // P) & 1) else 1)
-    return 0, 1
-
-
-def pfb_eps(w, PS, sigma):
-    """signed distance (rad) of w PS from 0 (sigma = +1) or 1/2 turn (sigma = -1), from the exact u64 w"""
-    r = (w * PS) % TWO64
-    return _signed(r if sigma > 0 else r - (1 << 63)) * (2.0 * math.pi / TWO64)
-
-
 def s1_route(ws, T, D, fmt, count, offset, variant=8, aligned=True):
     """Scheduler::run's variant choice, then launch_xd_fmt / try_xd_tma / try_xd_pfb / try_xd_pipe, for one chunk of a batch
     whose jobs share T, the chunk offset and the output count (one VFO set through one prototype); `aligned`: the chunk
@@ -149,49 +103,8 @@ def fir_offsets(sched, D):
     return offs
 
 
-def plan_of(oracle, ratio):
-    if ratio == 1:
-        return [(1, np.ones(1, np.float32))]
-    return [(D, np.asarray(oracle.decim_taps(ratio, k), np.float32)) for k, (D, T) in enumerate(oracle.decim_plan(ratio))]
-
-
 # ---------------------------------------------------------------------------------------------- float64 reference
-def rotate_f64(x, sched, offs, fs):
-    """the exact-phase translator: x (complex128, integer chunks already scaled) rotated by the u64 phase of each sample,
-    offs[c] the VFO offset chunk c was translated with"""
-    n = x.size
-    ph = np.empty(n, np.uint64)
-    phase, pos = 0, 0
-    for c, off in zip(sched, offs):
-        w = w_u64(off, fs)
-        ph[pos:pos + c] = np.uint64(phase) + np.uint64(w) * np.arange(c, dtype=np.uint64)
-        phase = (phase + w * c) % TWO64
-        pos += c
-    ang = (ph >> np.uint64(11)).astype(np.float64) * (2.0 * math.pi / 2.0 ** 53)
-    return x * np.exp(1j * ang)
-
-
-def drift_weights(T, PS):
-    """|floor(k / PS) - floor(T / (2 PS))|: how far tap k's drift is from the centred correction"""
-    k = np.arange(T)
-    return np.abs(k // PS - T // (2 * PS)).astype(np.float64)
-
-
-def stage1_f64(x, sched, offs, h, D, fs, eps=0.0, PS=0):
-    """exact-phase translator + DecimatingFIR from zero history (the specification form), with the per-component bound of
-    the module docstring; eps / PS: the largest filter-bank drift a chunk may carry (0: complex-tap builds only)"""
-    T = h.size
-    z = rotate_f64(x, sched, offs, fs)
-    hh = np.asarray(h, np.float64)
-    y = _corr(_hist(z, T - 1), hh)[::D]
-    ax = _hist(np.abs(x), T - 1)
-    A = math.sqrt(2.0) * _corr(ax, np.abs(hh))[::D]
-    b = (4 * T + 4 * PS + 40) * U * A + REF_FLOOR * np.abs(hh).sum() * 2.0 * float(np.abs(x).max(initial=0.0))
-    if PS:
-        b = b + math.sqrt(2.0) * abs(eps) * _corr(ax, np.abs(hh) * drift_weights(T, PS))[::D]
-    return y, b
-
-
+# (the translator, stage 1 and the filter-bank detection: f64_ref)
 def vfo_f64(oracle, x, sched, offs, fs, ratio, eps=0.0, PS=0):
     """RAW VFO with bw == outSR and outSR = fs / ratio: stage 1, then the plan's later DecimatingFIRs (the channel filter is
     the identity tap)"""
