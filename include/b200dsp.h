@@ -267,7 +267,7 @@ int b200_fe_wait(b200_fe* fe);
 /* number of kernels this handle has launched so far (bench.py's gpu_launches) */
 long long b200_fe_launch_count(b200_fe* fe);
 /* counters by name: "launches", "chunks", "s1_tma_launches" (stage-1 launches of this process that ran the TMA-fed
- * filter-bank kernel), "graphs" / "graph_hits" / "graph_misses" (launch lists captured / replayed / launched plainly),
+ * filter-bank kernel), "s1_f2_jobs" (VFO-chunks of this handle whose (4, 27) decimating FIR ran inside that kernel), "graphs" / "graph_hits" / "graph_misses" (launch lists captured / replayed / launched plainly),
  * "host_ns_plan" / "host_ns_fft" / "host_ns_run" / "host_ns_join" / "host_ns_stage1" / "host_ns_tail" (host time spent inside
  * b200_fe_submit since creation, by section, in ns), "fused_chains" (VFOs whose stages behind stage 1 are planned into one
  * k_tail_fused launch per chunk); -1 for an unknown key */

@@ -722,6 +722,7 @@ extern "C" long long b200_fe_stat(b200_fe* fe, const char* key) {
     if (!fe || !key) { return -1; }
     if (!strcmp(key, "launches")) { return fe->sch.launches; }
     if (!strcmp(key, "s1_tma_launches")) { return g_xd_tma_launches; }      // process-wide: stage-1 launches that took the TMA kernel
+    if (!strcmp(key, "s1_f2_jobs")) { return fe->sch.s1_f2_jobs; }
     if (!strcmp(key, "chunks")) { return (long long)fe->nsub; }
     // host time spent inside b200_fe_submit since creation, by section (ns)
     if (!strcmp(key, "host_ns_plan")) { return fe->host_ns[0]; }

@@ -206,6 +206,7 @@ int FirCStage::configure(const std::vector<float>& t, int decim_) {
     return upload_pm(t, decim, 1);
 }
 int FirCStage::plan(int n) {
+    prev_n_in = n_in;
     n_in = n;
     chunk_offset = offset;
     n_out = (offset < n) ? (n - offset + decim - 1) / decim : 0;
@@ -379,10 +380,19 @@ int FmIfStage::configure(int nbins) {
 }
 
 // ------------------------------------------------------------------ Chain
+// the decimating FIR that k_xd_tma can run as its ÷4 epilogue (kernels.cuh: XdJob::f2_out)
+static bool s1_f2_stage(const Stage* s) {
+    return s->kind == K_FIRC && s->in_es == 2 && ((const FirCStage*)s)->decim == XD_F2_D && ((const FirCStage*)s)->ntaps == XD_F2_T;
+}
 int Chain::finalize(int max_in, bool dbl_first, const FuseCfg* fuse) {
     if (st.empty()) { set_error("empty chain"); return B200_EINVAL; }
     int cap = max_in;
-    if (dbl_first && st.size() >= 2 && st[0]->kind == K_XD) { st[1]->dbl = true; }
+    if (dbl_first && st.size() >= 2 && st[0]->kind == K_XD) {
+        st[1]->dbl = true;
+        // stage 1 may produce the (4, 27) stage's outputs itself (Scheduler::run), where k_dfir_reg would run that stage: the
+        // stage after it is then fed by stage 1
+        if (st.size() >= 3 && s1_f2_stage(st[1].get()) && (fuse ? fuse->pre_reg : fcfg.pre_reg) > 0) { st[2]->dbl = true; }
+    }
     for (auto& s : st) {
         if (s->kind != K_XD) {
             int rc = s->alloc_in(cap);
@@ -617,8 +627,9 @@ void Chain::reset_state() {
 int Chain::unfuse_history() {
     for (auto& s : st) {
         if (s->fmid && s->hist > 0) {
-            // a fused-middle stage is never the double-buffered stage behind stage 1: its plain history is the head of inbuf
-            B200_CK(cudaMemcpy(s->inbuf.p, s->fh[s->fpar].p, (size_t)s->hist * s->in_es * sizeof(float), cudaMemcpyDeviceToDevice));
+            // its plain history is the head of the buffer the next chunk uses (of a double-buffered stage: not this chunk's)
+            B200_CK(cudaMemcpy(s->dbl ? s->other_base() : s->inbuf.as<float>(), s->fh[s->fpar].p, (size_t)s->hist * s->in_es * sizeof(float),
+                               cudaMemcpyDeviceToDevice));
         }
         s->fmid = false;
     }
@@ -630,7 +641,8 @@ int Chain::restage() {
     if (rc) { return rc; }
     for (auto& s : st) {
         if (s->fmid && s->hist > 0) {
-            B200_CK(cudaMemcpy(s->fh[s->fpar].p, s->inbuf.p, (size_t)s->hist * s->in_es * sizeof(float), cudaMemcpyDeviceToDevice));
+            B200_CK(cudaMemcpy(s->fh[s->fpar].p, s->dbl ? s->other_base() : s->inbuf.as<float>(), (size_t)s->hist * s->in_es * sizeof(float),
+                               cudaMemcpyDeviceToDevice));
         }
     }
     B200_CK(cudaDeviceSynchronize());      // device-to-device copies on the legacy stream
@@ -900,6 +912,13 @@ static int apply_pending_taps(FirCStage* f, cudaStream_t s) {
         B200_CK(cudaMemcpy(live_new + (size_t)(newH - keep) * f->in_es, live + (size_t)(oldH - keep) * f->in_es,
                            (size_t)keep * f->in_es * sizeof(float), cudaMemcpyDeviceToDevice));
     }
+    if (f->dbl && keep > 0) {
+        // and in front of the previous chunk's (empty) data in the other buffer, where stage 1's ÷4 epilogue looks for it
+        float* other_new = f->par ? nb2.as<float>() : nb.as<float>();
+        B200_CK(cudaMemcpy(other_new + (size_t)(newH - keep) * f->in_es, live + (size_t)(oldH - keep) * f->in_es,
+                           (size_t)keep * f->in_es * sizeof(float), cudaMemcpyDeviceToDevice));
+    }
+    f->n_in = 0;
     std::swap(f->inbuf.p, nb.p);
     std::swap(f->inbuf.bytes, nb.bytes);
     if (f->dbl) {
@@ -1152,12 +1171,23 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
     }
     // ---- stage 1: every raw-input chain, grouped by first-stage decimation so they share the IQ tile ----
     std::map<int, std::vector<XdStage*>> groups;
+    std::map<XdStage*, Chain*> chain_of;
     for (Chain* c : chains) {
         if (c->raw_input()) {
             XdStage* x = (XdStage*)c->st[0].get();
             groups[x->D].push_back(x);
+            chain_of[x] = c;
         }
     }
+    // The (4, 27) stage behind stage 1 is computed by k_xd_tma's ÷4 epilogue where it would otherwise run in k_dfir_reg (the
+    // epilogue has its arithmetic), the stage after it is double-buffered like the one stage 1 feeds, and the chunk needs no
+    // k_xd_edge patch of the stage-1 outputs.  Every other chunk -- a retune inside the tap window, another input format, a
+    // launch k_xd_tma declines -- stores the stage-1 outputs and runs k_dfir_reg, reading and writing the same history.
+    auto f2_stage = [&](Chain* c, const XdStage* x) -> FirCStage* {
+        if (fmt != FMT_CF32 || s1_variant < 8 || fuse.pre_reg <= 0 || x->chunk_retuned || c->st.size() < 3) { return nullptr; }
+        if (!s1_f2_stage(c->st[1].get()) || (tail_stream && !c->st[2]->dbl) || (c->fp.active && c->fp.beg <= 1)) { return nullptr; }
+        return (FirCStage*)c->st[1].get();
+    };
     for (auto& kv : groups) {
         std::vector<XdStage*>& g = kv.second;
         for (size_t b = 0; b < g.size(); b += B200_BATCH) {
@@ -1171,6 +1201,7 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
             p.in_scale = in_scale;
             p.QP = 1;
             p.njobs = (int)std::min<size_t>(B200_BATCH, g.size() - b);
+            const std::vector<float>* f2_taps = nullptr;
             for (int v = 0; v < p.njobs; v++) {
                 XdStage* x = g[b + v];
                 p.job[v].out = (float2*)x->out_ptr;
@@ -1193,6 +1224,18 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
                     p.job[v].edge_start = x->chunk_edge_start;
                 }
                 p.QP = std::max(p.QP, x->QP);
+                FirCStage* f = f2_stage(chain_of[x], x);
+                if (f && f->n_out > 0 && (!f2_taps || *f2_taps == f->htaps)) {       // one tap set per launch
+                    f2_taps = &f->htaps;
+                    memcpy(p.f2_taps, f->htaps.data(), sizeof(p.f2_taps));
+                    p.job[v].f2_out = (float2*)f->out_ptr;
+                    // the F2H stage-1 outputs in front of this chunk: the carry of the previous chunk's tail puts them at the
+                    // head of this chunk's buffer and may not have run yet; they are the last ones of the previous chunk's
+                    // [history | data], in the other buffer of a double-buffered stage
+                    p.job[v].f2_hist = (const float2*)(f->dbl ? f->other_base() + (size_t)2 * f->prev_n_in : f->base());
+                    p.job[v].f2_off = f->chunk_offset;
+                    p.job[v].f2_n = f->n_out;
+                }
             }
             // slots: pair VFOs whose complex taps are exact conjugates (offsets +f / -f, same real prototype, same
             // decimation phase): they share every multiply-accumulate of stage 1 (kernels.cuh: XdParams)
@@ -1265,9 +1308,15 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
                 if (g[b + v]->gpad_len < (p.D - 1) + (p.QP + 8) * p.D) { variant = 0; }
             }
             int nl = 0;
+            bool f2 = false;
             cudaEvent_t t1 = timer_begin(0, stream);
-            cudaError_t e = launch_xlate_decim(p, fmt, variant, stream, &nl);
+            cudaError_t e = launch_xlate_decim(p, fmt, variant, stream, &nl, &f2);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_xlate_decim"); }
+            for (int v = 0; v < p.njobs; v++) {
+                Chain* c = chain_of[g[b + v]];
+                if (c->st.size() >= 2 && c->st[1]->kind == K_FIRC) { ((FirCStage*)c->st[1].get())->s1_fused = f2 && p.job[v].f2_out; }
+                if (f2 && p.job[v].f2_out) { s1_f2_jobs++; }
+            }
             if (t1) { B200_CK(cudaEventRecord(t1, stream)); }
             trace_mark("stage1 done", stream);
             e = launch_xd_edge(p, fmt, stream, &nl);
@@ -1347,7 +1396,7 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
             for (Chain* c : chains) {
                 if (!c->fp.active || lvl >= c->fp.beg) { continue; }
                 FirCStage* f = (FirCStage*)c->st[lvl].get();
-                if (f->n_out <= 0) { continue; }
+                if (f->n_out <= 0 || f->s1_fused) { continue; }
                 int rc = dfr_push(f);
                 if (rc) { return rc; }
             }
@@ -1514,7 +1563,7 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
             case K_XD: break;
             case K_FIRC: {
                 FirCStage* f = (FirCStage*)s;
-                if (f->n_out <= 0) { break; }
+                if (f->n_out <= 0 || f->s1_fused) { break; }
                 if (dfr_ok(f)) { rc = dfr_push(f); break; }
                 if (fuse.pre_reg > 0 && f->decim == 1 && f->in_es == 2 && f->ntaps <= 2000 && f->chunk_offset == 0) {
                     FirJob& jr = fpr.job[fpr.njobs++];

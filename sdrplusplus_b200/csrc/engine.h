@@ -105,6 +105,8 @@ struct XdStage : Stage {
 
 struct FirCStage : Stage {
     int ntaps = 1, decim = 1, offset = 0, chunk_offset = 0;
+    int prev_n_in = 0;           // n_in of the previous chunk (where its last ntaps-1 inputs lie in the other buffer of a dbl stage)
+    bool s1_fused = false;       // this chunk: stage 1 computed this stage's outputs (k_xd_tma's ÷4 epilogue)
     DevBuf taps;
     std::vector<float> htaps;    // host copy of the taps in use
     std::vector<float> pending;  // FIR::setTaps applied at the next chunk boundary
@@ -114,7 +116,7 @@ struct FirCStage : Stage {
     // one output more than plan() can give: with decim 1 the stage is 1:1 (the radio's 300 Hz high-pass), and the front end keeps a
     // VFO's bound the same when that filter is switched on or off (api.cpp: vfo_out_bound)
     int max_out(int n) const override { return (n + decim - 1) / decim + 1; }
-    void reset_state() override { offset = 0; }
+    void reset_state() override { offset = 0; n_in = 0; prev_n_in = 0; }
 };
 
 struct PolyStage : Stage {
@@ -311,6 +313,7 @@ struct Scheduler {
     cudaStream_t out_stream() const { return tail_stream ? tail_stream : stream; }
     int enable_overlap(cudaStream_t tail);
     long long launches = 0;
+    long long s1_f2_jobs = 0;    // VFO-chunks whose (4, 27) stage stage 1 computed (k_xd_tma's ÷4 epilogue; b200_fe_stat "s1_f2_jobs")
     // launch-list replay (LaunchRec): -1 = for chunks up to graph_max_count samples, 0 = never, 1 = always
     int graph_tails = -1;
     int graph_max_count = 1 << 30;

@@ -917,30 +917,32 @@ void kernels_set_xd_tma_stages(int n) { g_xd_tma_stages = (n == 3) ? 3 : 2; }
 static int g_xd_tma_diag = 0;     // XtGeom::diag (measurement only)
 void kernels_set_xd_tma_diag(int v) { g_xd_tma_diag = v & 3; }
 template <int LOGD, int QC, int PS, int MT, int NST>
-static cudaError_t launch_xd_tma_n(const XdParams& p, const XtGeom& g, const CUtensorMap& tm, cudaStream_t s) {
+static cudaError_t launch_xd_tma_n(const XdParams& p, const XtGeom& g, const CUtensorMap& tm, int grid, cudaStream_t s) {
     using Lay = XtLay<LOGD, QC, MT>;
-    const size_t smem = (size_t)NST * Lay::STAGE + ((size_t)B200_BATCH * (PS + 16) + (size_t)Lay::NW * B200_BATCH * 4) * sizeof(float2) +
-                        2 * NST * sizeof(unsigned long long) + 1024;
+    // ring + phasor tables of the launch's jobs + barriers + the ÷4 epilogue's carried window (F2H outputs per job, only with
+    // the epilogue).  At config 2 (8 VFOs, PS 10) that is 141.3 KiB: with a pass-1 FFT CTA of 8 (82.1 KiB) and 2 x 1 KiB
+    // reserved it stays within the SM's 228 KiB
+    auto bytes = [&](int nj, bool f2) {
+        return (size_t)NST * Lay::STAGE + ((size_t)nj * (PS + 16) + (size_t)Lay::NW * nj * 4 + (f2 ? (size_t)nj * Lay::F2H : 0)) * sizeof(float2) +
+               2 * NST * sizeof(unsigned long long) + 1024;
+    };
+    const size_t smem = bytes(p.njobs, g.f2 != 0);
     if ((int)smem > kernels_max_smem_optin()) { return cudaErrorInvalidValue; }
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = set_smem(k_xd_tma<LOGD, QC, PS, MT, NST>, smem);
+        cudaError_t e = set_smem(k_xd_tma<LOGD, QC, PS, MT, NST>, bytes(B200_BATCH, true));
         if (e != cudaSuccess) { return e; }
         attr_set = true;
     }
-    // one persistent CTA per SM, or fewer (kernels_set_xd_tma_ctas): the SMs left out are free for the kernels of the other streams
-    int grid = num_sms();
-    if (g_xd_tma_ctas > 0 && g_xd_tma_ctas < grid) { grid = g_xd_tma_ctas; }
-    if (grid > g.ntiles) { grid = g.ntiles; }
     k_xd_tma<LOGD, QC, PS, MT, NST><<<grid, (Lay::NW + 1) * 32, smem, s>>>(p, g, tm);
     g_xd_tma_launches++;
     return cudaGetLastError();
 }
 template <int LOGD, int QC, int PS, int MT>
-static cudaError_t launch_xd_tma_t(const XdParams& p, const XtGeom& g, const CUtensorMap& tm, cudaStream_t s) {
-    return g_xd_tma_stages == 3 ? launch_xd_tma_n<LOGD, QC, PS, MT, 3>(p, g, tm, s) : launch_xd_tma_n<LOGD, QC, PS, MT, 2>(p, g, tm, s);
+static cudaError_t launch_xd_tma_t(const XdParams& p, const XtGeom& g, const CUtensorMap& tm, int grid, cudaStream_t s) {
+    return g_xd_tma_stages == 3 ? launch_xd_tma_n<LOGD, QC, PS, MT, 3>(p, g, tm, grid, s) : launch_xd_tma_n<LOGD, QC, PS, MT, 2>(p, g, tm, grid, s);
 }
-static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err) {
+static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err, bool* f2) {
     const int D = p.D, PS = p.pfb_ps;
     if ((PS != 8 && PS != 10) || (D != 32 && D != 64) || !p.taps_host) { return false; }
     if (((uintptr_t)p.in & 15) != 0) { return false; }
@@ -979,8 +981,21 @@ static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err) {
     const long long avail = (long long)p.count - g.org;
     g.rows_tma = avail > 0 ? (int)(avail / (2 * D)) : 0;
     const int MT = (D == 32) ? 256 : 128;
-    g.ntiles = cdiv((long long)g.cj + p.job[0].n_out - jmin, MT);
+    g.jend = (long long)g.cj + p.job[0].n_out;
     if (g.rows_tma < 8) { return false; }
+    // contiguous runs of whole tiles, one per persistent CTA (one per SM, or fewer: kernels_set_xd_tma_ctas leaves SMs free for
+    // the kernels of the other streams).  With the ÷4 epilogue every CTA but the first also filters the 32 outputs in front of
+    // its run; the run is then 32 short of its tiles, and no CTA does more tiles than without the epilogue plus the halo.
+    for (int v = 0; v < p.njobs; v++) {
+        if (p.job[v].f2_out && !g.diag) { g.f2 = 1; }
+    }
+    g.halo = g.f2 ? 32 : 0;
+    int grid = num_sms();
+    if (g_xd_tma_ctas > 0 && g_xd_tma_ctas < grid) { grid = g_xd_tma_ctas; }
+    const long long nblk = g.jend - jmin;
+    const long long tiles_per_cta = cdiv(cdiv(nblk, grid) + g.halo, MT);
+    g.run = (int)(tiles_per_cta * MT - g.halo);
+    grid = (int)cdiv(nblk, g.run);
     CUtensorMap tm;
     const cuuint64_t gdim[2] = { (cuuint64_t)(4 * D), (cuuint64_t)g.rows_tma };
     const cuuint64_t gstr[1] = { (cuuint64_t)(4 * D) * sizeof(float) };
@@ -993,7 +1008,8 @@ static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err) {
     if (r != CUDA_SUCCESS) { return false; }
 #define XT_CASE(LD, Q, MTV)                                                                    \
     if (D == (1 << LD) && QC == Q) {                                                           \
-        *err = (PS == 10) ? launch_xd_tma_t<LD, Q, 10, MTV>(p, g, tm, s) : launch_xd_tma_t<LD, Q, 8, MTV>(p, g, tm, s); \
+        *err = (PS == 10) ? launch_xd_tma_t<LD, Q, 10, MTV>(p, g, tm, grid, s) : launch_xd_tma_t<LD, Q, 8, MTV>(p, g, tm, grid, s); \
+        *f2 = g.f2 != 0;                                                                       \
         return true;                                                                           \
     }
     XT_CASE(5, 5, 256) XT_CASE(6, 5, 128) XT_CASE(6, 6, 128) XT_CASE(6, 7, 128)
@@ -1002,14 +1018,14 @@ static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err) {
 }
 
 template <int FMT>
-static cudaError_t launch_xd_fmt(const XdParams& p, int variant, cudaStream_t s, int* nlaunch) {
+static cudaError_t launch_xd_fmt(const XdParams& p, int variant, cudaStream_t s, int* nlaunch, bool* f2) {
     int max_out = 0;
     for (int v = 0; v < p.njobs; v++) { max_out = p.job[v].n_out > max_out ? p.job[v].n_out : max_out; }
     if (max_out <= 0) { return cudaSuccess; }
     const int D = p.D;
     if (variant >= 7) {
         cudaError_t e = cudaSuccess;
-        if (variant >= 8 && FMT == FMT_CF32 && p.pfb_ps > 0 && try_xd_tma(p, s, &e)) {
+        if (variant >= 8 && FMT == FMT_CF32 && p.pfb_ps > 0 && try_xd_tma(p, s, &e, f2)) {
             if (nlaunch) { (*nlaunch)++; }
             return e;
         }
@@ -1035,10 +1051,11 @@ static cudaError_t launch_xd_fmt(const XdParams& p, int variant, cudaStream_t s,
     return cudaGetLastError();
 }
 
-cudaError_t launch_xlate_decim(const XdParams& p, int fmt, int variant, cudaStream_t s, int* nlaunch) {
-    if (fmt == FMT_CF32) { return launch_xd_fmt<FMT_CF32>(p, variant, s, nlaunch); }
-    if (fmt == FMT_CS16) { return launch_xd_fmt<FMT_CS16>(p, variant, s, nlaunch); }
-    return launch_xd_fmt<FMT_CS8>(p, variant, s, nlaunch);
+cudaError_t launch_xlate_decim(const XdParams& p, int fmt, int variant, cudaStream_t s, int* nlaunch, bool* f2) {
+    *f2 = false;
+    if (fmt == FMT_CF32) { return launch_xd_fmt<FMT_CF32>(p, variant, s, nlaunch, f2); }
+    if (fmt == FMT_CS16) { return launch_xd_fmt<FMT_CS16>(p, variant, s, nlaunch, f2); }
+    return launch_xd_fmt<FMT_CS8>(p, variant, s, nlaunch, f2);
 }
 
 

@@ -30,7 +30,16 @@ struct XdJob {
     const unsigned long long* hphase;   // T-1 phases (turns * 2^64) of the history samples
     int edge_start;         // newest retune boundary, chunk-relative (<= 0)
     int retuned;
+    // ÷4 epilogue of k_xd_tma (xd_tma.cuh): when f2_out is set and the TMA kernel runs, the job's next stage, a (4, 27)
+    // decimating FIR, is computed there: f2_out[j] = sum_k f2_taps[k] * x[f2_off + 4 j + k], x = the 26 stage-1 outputs in
+    // front of the chunk (f2_hist) followed by this chunk's.  Only the last 26 stage-1 outputs are stored to `out` (the
+    // stage's history, carried as on the other path).  Every other build ignores these fields and stores all of `out`.
+    float2* f2_out;
+    const float2* f2_hist;
+    int f2_off, f2_n;
 };
+#define XD_F2_D 4
+#define XD_F2_T 27
 struct XdParams {
     const void* in;         // chunk data (format FMT), chunk-relative index 0
     const float2* hist;     // last `hist_len` samples before the chunk (cf32), hist[hist_len + i] for i < 0
@@ -49,6 +58,7 @@ struct XdParams {
     int pfb_ps, pfb_sigma;
     float in_scale;         // integer formats: sample = (float)x * in_scale
     const float* taps_host; // HOST copy of the real prototype taps shared by the jobs of a filter-bank launch (launcher only)
+    float f2_taps[XD_F2_T]; // taps of the ÷4 epilogue, shared by every job that has one
     XdJob job[B200_BATCH];
 };
 
@@ -346,7 +356,8 @@ struct FftPlanDev {
 };
 
 // launch wrappers (return cudaGetLastError())
-cudaError_t launch_xlate_decim(const XdParams& p, int fmt, int variant, cudaStream_t s, int* nlaunch);
+// *f2 = true when the launch ran the ÷4 epilogue of the jobs that carry one (k_xd_tma); false: every job stored `out`
+cudaError_t launch_xlate_decim(const XdParams& p, int fmt, int variant, cudaStream_t s, int* nlaunch, bool* f2);
 cudaError_t launch_xd_edge(const XdParams& p, int fmt, cudaStream_t s, int* nlaunch);
 cudaError_t launch_fir_c(const FirParams& p, cudaStream_t s);
 cudaError_t launch_fir_reg(const FirParams& p, cudaStream_t s);            // every job: decimation 1

@@ -17,6 +17,11 @@
 //     the real taps come from the kernel parameter block (constant bank), not from shared memory.
 // Rows are cut at a 128-byte aligned origin org' <= org; the s = org - org' samples in front of a window are covered
 // by s leading zero taps: the accumulator class of window position p is p mod PS, the tap it carries is k = p - s.
+//
+// ÷4 epilogue (XdJob::f2_out): when a VFO's next stage is the (4, 27) decimating FIR of the reference's plans, the kernel
+// runs it too, so the stage-1 outputs (4x the bytes of the (4, 27) outputs) never make a round trip through memory.  The
+// tile's stage-1 outputs are staged in the ring slot the tile arrived in (held until the epilogue has read it), behind
+// the 26 outputs carried from the previous tile of the CTA's contiguous run; the first tile of a run recomputes them.
 #pragma once
 #include <cuda.h>
 
@@ -26,7 +31,13 @@
 struct XtGeom {
     float g[XT_MAXTAPS];      // signed real taps by window position p = q*D + r:  sigma^floor(k/PS) h[k], k = p - s
     long long jmin;           // block index (relative to the row origin) of the first tile's first output, even
-    int ntiles;
+    long long jend;           // one past the block index of the last output
+    // CTA b owns the outputs of blocks [jmin + b*run, jmin + (b+1)*run) and walks them in consecutive tiles, so that the ÷4
+    // epilogue carries its window from tile to tile.  With the epilogue, every CTA but the first starts `halo` outputs early
+    // and only filters those: the ÷4 windows of its first outputs reach 26 stage-1 outputs back.  run, halo: multiples of 16,
+    // so that every output keeps the coarse-phase grouping (PHW) it has in a launch without the epilogue.
+    int run, halo;
+    int f2;                   // some job has a ÷4 epilogue (XdJob::f2_out)
     int org;                  // sample index of row 0, phase 0 (chunk-relative; may be negative: history)
     int s;                    // leading zero taps
     int cj;                   // window of output m starts in block cj + m
@@ -68,7 +79,14 @@ struct XtLay {
     static constexpr int REGION = NR * 128;
     static constexpr int STAGE = NSEG * 2 * REGION;
     static constexpr int NW = MT / 64;                                   // consumer warps
+    // ÷4 epilogue: per job, the 26 carried stage-1 outputs and the MT of the tile, staged in the ring slot the tile came in,
+    // one pad entry per 16 (a thread reads the 39-entry window of four ÷4 outputs; neighbouring threads are 16 apart)
+    static constexpr int F2H = XD_F2_T - 1;
+    static constexpr int F2P = (F2H + MT) + (F2H + MT) / 16 + 2;
+    static_assert(B200_BATCH * F2P * 8 <= STAGE, "the epilogue's staging fits in one ring slot");
+    static_assert(MT % 16 == 0, "whole groups of four ÷4 outputs per tile");
 };
+__device__ __forceinline__ int xt_f2_pad(int i) { return i + (i >> 4); }
 
 // decimation-phase pairs [RP0, RP1) of a tile -- they all lie in ONE 128-byte segment (8 pairs per segment), whose two parity
 // regions start at sb -- into the 2 x PS class sums of a lane.  Every index is a compile-time constant: taps from the constant
@@ -117,12 +135,17 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
     const unsigned sbase = ((unsigned)__cvta_generic_to_shared(xt_smem) + 1023u) & ~1023u;
     unsigned char* const gbase = xt_smem + (sbase - (unsigned)__cvta_generic_to_shared(xt_smem));
     float2* C = reinterpret_cast<float2*>(gbase + XT_STAGES * STAGE);    // [njobs][PS]  e^{j w_v ((b - s) mod PS)}
-    float2* TL = C + (size_t)B200_BATCH * PS;                            // [njobs][16]  e^{j w_v D j}
-    float2* PHW = TL + (size_t)B200_BATCH * 16;                          // [NW][njobs][4] per warp and tile: coarse phase
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(PHW + (size_t)NW * B200_BATCH * 4);
+    float2* TL = C + (size_t)p.njobs * PS;                               // [njobs][16]  e^{j w_v D j}
+    float2* PHW = TL + (size_t)p.njobs * 16;                             // [NW][njobs][4] per warp and tile: coarse phase
+    unsigned long long* bars = reinterpret_cast<unsigned long long*>(PHW + (size_t)NW * p.njobs * 4);
     const unsigned bar0 = (unsigned)__cvta_generic_to_shared(bars);     // full[s] = bar0 + 8 s, empty[s] = bar0 + 8 (NSLOT + s)
+    float2* H = reinterpret_cast<float2*>(bars + 2 * NSLOT);              // [njobs][F2H] ÷4 epilogue: carried stage-1 outputs
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    // this CTA's run of tiles (XtGeom::run)
+    const long long own0 = g.jmin + (long long)blockIdx.x * g.run;
+    const long long own1 = own0 + g.run < g.jend ? own0 + g.run : g.jend;
+    const long long first = own0 - (blockIdx.x > 0 ? g.halo : 0);
 
     if (tid == 0) {
         for (int s = 0; s < NSLOT; s++) {
@@ -144,6 +167,14 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
             const int v = idx >> 4, j = idx & 15;
             TL[idx] = phasor_u64(p.job[v].w * (unsigned long long)((long long)j * D));
         }
+        if (g.f2) {
+            // the stage-1 outputs in front of the first tile: only the first CTA reads them (from the stage's history)
+            for (int idx = tid; idx < p.njobs * Lay::F2H; idx += NW * 32) {
+                const int v = idx / Lay::F2H, i = idx - v * Lay::F2H;
+                const long long m = first - g.cj - Lay::F2H + i;
+                H[idx] = (p.job[v].f2_out && m >= -Lay::F2H && m < 0) ? p.job[v].f2_hist[Lay::F2H + m] : make_float2(0.f, 0.f);
+            }
+        }
         asm volatile("bar.sync 1, %0;\n" ::"n"(NW * 32) : "memory");
     }
 
@@ -156,8 +187,7 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
         if (lane == 0 && !(g.diag & 2)) {
             const unsigned long long pol = xt_policy_evict_first();
             int it = 0;                                                  // slot steps issued so far
-            for (int tile = blockIdx.x; tile < g.ntiles; tile += gridDim.x) {
-                const long long J0 = g.jmin + (long long)tile * MT;
+            for (long long J0 = first; J0 < own1; J0 += MT) {
                 const int row0 = (int)(J0 >> 1);
                 // every tile comes in through the TMA engine; rows outside the tensor (negative: stream history in front of
                 // the chunk; past its last full super-row: the ragged end) arrive zero-filled and are patched by the consumers
@@ -189,8 +219,7 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
         aoff[qh] = row * 128u + ((row & 7u) << 4);
     }
     int it = 0;                                     // tiles consumed so far (the producer's sequence)
-    for (int tile = blockIdx.x; tile < g.ntiles; tile += gridDim.x) {
-        const long long J0 = g.jmin + (long long)tile * MT;
+    for (long long J0 = first; J0 < own1; J0 += MT) {
         // coarse phase table of this warp's 64 outputs: entry (job, i) = phase at output jl0 + 16 i, drift-centred
         {
             for (int e = lane; e < p.njobs * 4; e += 32) {
@@ -201,7 +230,7 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
                 unsigned long long dr = Jv.w * (unsigned long long)PS;
                 if (p.pfb_sigma < 0) { dr -= 0x8000000000000000ULL; }
                 const long long corr = (long long)dr * (long long)(Jv.T / (2 * PS));
-                PHW[(warp * B200_BATCH + vv) * 4 + i] = phasor_u64(Jv.phase0 + Jv.w * (unsigned long long)im0 + (unsigned long long)corr);
+                PHW[(warp * p.njobs + vv) * 4 + i] = phasor_u64(Jv.phase0 + Jv.w * (unsigned long long)im0 + (unsigned long long)corr);
             }
         }
         const bool fast = tile_fast(J0);
@@ -250,18 +279,45 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
             }
         }
         static_assert(NSEG == 2 || NSEG == 4, "D = 32 or 64");
-        // the tile is consumed: hand it back to the producer before the (register-only) combination
         __syncwarp();
-        if (lane == 0 && !(g.diag & 2)) { xt_mbar_arrive(bar0 + 8 * (NSLOT + sl)); }
+        if (!g.f2) {
+            // the tile is consumed: hand it back to the producer before the (register-only) combination.  Patched samples were
+            // written through the generic proxy: order them before the TMA engine's next write into the slot
+            if (!fast) { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); __syncwarp(); }
+            if (lane == 0 && !(g.diag & 2)) { xt_mbar_arrive(bar0 + 8 * (NSLOT + sl)); }
+            if (g.diag & 1) { continue; }
+        }
+        else {
+            // the slot becomes the epilogue's staging once every warp has read its part of the tile
+            asm volatile("bar.sync 1, %0;\n" ::"n"(NW * 32) : "memory");
+        }
+        float2* const stg = reinterpret_cast<float2*>(gbase + sl * SLOT);
+        if (g.f2) {
+            for (int idx = tid; idx < p.njobs * Lay::F2H; idx += NW * 32) {
+                const int v = idx / Lay::F2H, i = idx - v * Lay::F2H;
+                stg[v * Lay::F2P + xt_f2_pad(i)] = H[idx];
+            }
+        }
 
-        if (g.diag & 1) { continue; }
         // ---- combine per slot (a VFO, or a +f / -f pair sharing A = sum cos*S and B = sum sin*S), rotate, store ----
         const long long m0 = J0 + jl - (long long)g.cj;
         const int nout = p.job[0].n_out;                       // every job of a filter-bank launch has the same length
-        const bool ok0 = m0 >= 0 && m0 < nout, ok1 = (m0 + 1) >= 0 && (m0 + 1) < nout;
+        // outputs of this CTA's run (the halo in front of it and the tail past its end belong to its neighbours)
+        const bool own0k = J0 + jl >= own0 && J0 + jl < own1, own1k = J0 + jl + 1 >= own0 && J0 + jl + 1 < own1;
+        const bool ok0 = own0k && m0 >= 0 && m0 < nout, ok1 = own1k && (m0 + 1) >= 0 && (m0 + 1) < nout;
         const int ih = (2 * lane) >> 4, il = (2 * lane) & 15;
-        for (int sl = 0; sl < p.nslots; sl++) {
-            const int ja = p.slot_a[sl], jb = p.slot_b[sl];
+        // stage-1 output y of job v at m: to the ÷4 staging, and to `out` where the next stage's history needs it
+        auto put = [&](int v, long long m, bool ok, float2 y, float2* out) {
+            const XdJob& Jv = p.job[v];
+            if (g.f2 && Jv.f2_out) {
+                // m < 0 only in the first CTA's first tile, when the first output's block is odd: the value of the history
+                stg[v * Lay::F2P + xt_f2_pad(Lay::F2H + (int)(m - m0) + jl)] = m >= 0 ? y : Jv.f2_hist[Lay::F2H + m];
+                if (ok && m >= nout - Lay::F2H) { *out = y; }
+            }
+            else if (ok) { *out = y; }
+        };
+        for (int sv = 0; sv < p.nslots; sv++) {
+            const int ja = p.slot_a[sv], jb = p.slot_b[sv];
             float2 A0 = make_float2(0.f, 0.f), B0 = A0, A1 = A0, B1 = A0;
             const float2* cv = C + ja * PS;
 #pragma unroll
@@ -273,19 +329,63 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
                 B1 = ffma2(make_float2(c.y, c.y), S[1][a], B1);
             }
             {
-                const float2 pc = PHW[(warp * B200_BATCH + ja) * 4 + ih];
+                const float2 pc = PHW[(warp * p.njobs + ja) * 4 + ih];
                 const float2 p0 = cmulf(pc, TL[ja * 16 + il]), p1 = cmulf(pc, TL[ja * 16 + il + 1]);
                 float2* out = p.job[ja].out + m0;
-                if (ok0) { out[0] = cmulf(make_float2(A0.x - B0.y, A0.y + B0.x), p0); }
-                if (ok1) { out[1] = cmulf(make_float2(A1.x - B1.y, A1.y + B1.x), p1); }
+                put(ja, m0, ok0, cmulf(make_float2(A0.x - B0.y, A0.y + B0.x), p0), out);
+                put(ja, m0 + 1, ok1, cmulf(make_float2(A1.x - B1.y, A1.y + B1.x), p1), out + 1);
             }
             if (jb >= 0) {
-                const float2 pc = PHW[(warp * B200_BATCH + jb) * 4 + ih];
+                const float2 pc = PHW[(warp * p.njobs + jb) * 4 + ih];
                 const float2 p0 = cmulf(pc, TL[jb * 16 + il]), p1 = cmulf(pc, TL[jb * 16 + il + 1]);
                 float2* out = p.job[jb].out + m0;
-                if (ok0) { out[0] = cmulf(make_float2(A0.x + B0.y, A0.y - B0.x), p0); }      // conjugate coefficients
-                if (ok1) { out[1] = cmulf(make_float2(A1.x + B1.y, A1.y - B1.x), p1); }
+                put(jb, m0, ok0, cmulf(make_float2(A0.x + B0.y, A0.y - B0.x), p0), out);      // conjugate coefficients
+                put(jb, m0 + 1, ok1, cmulf(make_float2(A1.x + B1.y, A1.y - B1.x), p1), out + 1);
             }
+        }
+        if (g.f2) {
+            asm volatile("bar.sync 1, %0;\n" ::"n"(NW * 32) : "memory");
+            // ---- ÷4 epilogue: a thread computes four consecutive outputs of one job from a 39-entry window in registers,
+            //      with the tap order and arithmetic of k_dfir_reg ----
+            constexpr int NG = MT / 16;                        // groups of four outputs per job and tile
+            const long long t0 = J0 - g.cj;                    // stage-1 index of the tile's first output (staging entry F2H)
+            for (int task = tid; task < p.njobs * NG; task += NW * 32) {
+                const int v = task / NG, gi = task - v * NG;
+                const XdJob& Jv = p.job[v];
+                if (!Jv.f2_out) { continue; }
+                // first output whose window ends inside the tile: f2_off + 4 j >= t0
+                const long long d = t0 - Jv.f2_off;
+                const long long jt0 = d >= 0 ? (d + 3) / 4 : -((-d) / 4);
+                const int b = (int)(Jv.f2_off + 4 * jt0 - t0) + 16 * gi;
+                const float2* w = stg + v * Lay::F2P;
+                float2 x[3 * XD_F2_D + XD_F2_T];
+#pragma unroll
+                for (int i = 0; i < 3 * XD_F2_D + XD_F2_T; i++) { x[i] = w[xt_f2_pad(b + i)]; }
+                float2 acc[4];
+#pragma unroll
+                for (int i = 0; i < 4; i++) { acc[i] = make_float2(0.0f, 0.0f); }
+#pragma unroll
+                for (int k = 0; k < XD_F2_T; k++) {
+                    const float h = p.f2_taps[k];
+#pragma unroll
+                    for (int i = 0; i < 4; i++) { acc[i] = ffma2(make_float2(h, h), x[i * XD_F2_D + k], acc[i]); }
+                }
+#pragma unroll
+                for (int i = 0; i < 4; i++) {
+                    const long long j = jt0 + 4 * gi + i;
+                    const long long J = Jv.f2_off + XD_F2_D * j + g.cj;   // block of the window's last stage-1 output
+                    if (j >= 0 && j < Jv.f2_n && J >= own0 && J < own1) { Jv.f2_out[j] = acc[i]; }
+                }
+            }
+            // the last F2H stage-1 outputs of the tile are the window's start in the next one
+            for (int idx = tid; idx < p.njobs * Lay::F2H; idx += NW * 32) {
+                const int v = idx / Lay::F2H, i = idx - v * Lay::F2H;
+                H[idx] = stg[v * Lay::F2P + xt_f2_pad(MT + i)];
+            }
+            // the staging is read: the slot goes back to the producer, its generic-proxy writes ordered before the next TMA write
+            asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+            __syncwarp();
+            if (lane == 0) { xt_mbar_arrive(bar0 + 8 * (NSLOT + sl)); }
         }
         __syncwarp();                                          // PHW is rewritten for the next tile
     }
