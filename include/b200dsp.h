@@ -248,6 +248,21 @@ int b200_fe_set_vfo_config(b200_fe* fe, int id, const b200_vfo_cfg* cfg);
 #define B200_IQ_I32  4
 int b200_fe_bind_iq(b200_fe* fe, int sample_type, float scalar);   /* returns an id */
 int b200_fe_unbind_iq(b200_fe* fe, int id);
+/* BroadcastFM's rdsOut on a front-end VFO, the radio's "Decode RDS" (decoder_modules/radio/src/demodulators/wfm.h:118-119,
+ * broadcast_fm.h:121-142,165-170,196-202): the RDS branch hangs off the discriminator of VFO vfo_id (B200_DEMOD_WFM or
+ * B200_DEMOD_WFM_STEREO, at most one RDS output each), whose audio goes on.  Returns an id of the VFO id space: its records
+ * travel in b200_outputs.vfo_out[id] exactly as those of a B200_DEMOD_WFM_RDS_BITS VFO at the same offset and settings --
+ * vfo_cap[id] counts records, vfo_count[id] is filled by b200_fe_wait (b200_fe_process, b200_shard_wait), b200_fe_vfo_max_out
+ * bounds them (b200_rds_demod_max_out of the branch's 5 kS/s samples); b200_fe_vfo_count counts RDS outputs.  The work in
+ * front of the discriminator runs once for both, and the branch's stages join the chunk's batched launches.
+ * As setRDSOut's reset(): at the first chunk after a bind or an unbind the parent's discriminator history, stereo stage and
+ * 15 kHz low-pass restart; RxVFO, IF chain and AF chain keep their state (a bind before the first chunk changes nothing of the
+ * audio).  The branch starts fresh at its first bind; an unbind parks it with its state (translator phase, resampler
+ * histories, RDSDemod), a later bind resumes it, b200_fe_reset clears it.
+ * B200_EINVAL: a parent of another mode, a second output, an RDS id passed to the VFO setters, b200_fe_remove_vfo or
+ * b200_fe_unbind_iq; B200_ESTATE: b200_fe_remove_vfo on a VFO that has an RDS output, b200_fe_set_decimation after a bind. */
+int b200_fe_bind_rds(b200_fe* fe, int vfo_id);        /* returns an id */
+int b200_fe_unbind_rds(b200_fe* fe, int id);
 int b200_fe_vfo_count(b200_fe* fe);
 /* upper bound of output samples one chunk of `count` input samples can produce for VFO id */
 int b200_fe_vfo_max_out(b200_fe* fe, int id, int count);

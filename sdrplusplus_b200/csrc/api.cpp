@@ -257,8 +257,14 @@ struct VfoSlot {
     // an IQ tap (b200_fe_bind_iq) instead of a VFO: no chain, the chunk's effective stream in sample type tap_type (B200_IQ_*)
     int tap_type = -1;
     float tap_scalar = 0.0f;
+    // an RDS output (b200_fe_bind_rds): `chain` is the branch behind the discriminator of VFO rds_parent, with rds / rds_rec as
+    // for WFM_RDS_BITS.  On the parent: rds_child is its bound output, rds_parked the branch an unbind left, with its state.
+    int rds_parent = -1;
+    int rds_child = -1;
+    std::unique_ptr<VfoSlot> rds_parked;
 };
 static bool is_tap(const VfoSlot* v) { return v->tap_type >= 0; }
+static bool is_rds_out(const VfoSlot* v) { return v->rds_parent >= 0; }
 // bytes per complex sample of an IQ tap's output (interleaved I, Q)
 static size_t iq_tap_bytes(int type) {
     return type == B200_IQ_CF32 || type == B200_IQ_I32 ? 8 : (type == B200_IQ_I16 ? 4 : 2);
@@ -493,6 +499,18 @@ static bool vfo_has_audio(const b200_vfo_cfg& c) {
     return c.demod != B200_DEMOD_RAW && c.demod != B200_DEMOD_WFM_RDS && c.demod != B200_DEMOD_WFM_RDS_BITS;
 }
 
+// RDSDemod behind a chain that gives at most n_max 5 kS/s samples per chunk, and its record buffer
+static int add_rds_demod(b200_fe* fe, VfoSlot* v, int n_max) {
+    if (!fe->rds_count && cudaMallocHost((void**)&fe->rds_count, sizeof(int) * FE_SLOTS * B200_MAX_VFOS) != cudaSuccess) {
+        fe->rds_count = nullptr;
+        return cuda_fail(cudaGetLastError(), "cudaMallocHost");
+    }
+    v->rds = std::make_unique<RdsCore>();
+    int rc = v->rds->create(nullptr);
+    if (rc) { return rc; }
+    return v->rds_rec.alloc((size_t)b200_rds_demod_max_out(n_max) * sizeof(RdsSym), false);
+}
+
 static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
     const b200_vfo_cfg& c = v->cfg;
     int rc = v->chain.add_rxvfo(fe->fs_eff, c.out_samplerate, c.bandwidth, c.offset);
@@ -543,20 +561,19 @@ static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
         if ((rc = v->chain.add_fir_c(std::vector<float>{ 1.0f }, 1))) { return rc; }
     }
     if ((rc = v->chain.finalize(fe->max_eff, ov, &fe->sch.fuse))) { return rc; }
-    if (c.demod == B200_DEMOD_WFM_RDS_BITS) {
-        if (!fe->rds_count && cudaMallocHost((void**)&fe->rds_count, sizeof(int) * FE_SLOTS * B200_MAX_VFOS) != cudaSuccess) {
-            fe->rds_count = nullptr;
-            return cuda_fail(cudaGetLastError(), "cudaMallocHost");
-        }
-        v->rds = std::make_unique<RdsCore>();
-        if ((rc = v->rds->create(nullptr))) { return rc; }
-        return v->rds_rec.alloc((size_t)b200_rds_demod_max_out(v->chain.max_out(fe->max_eff)) * sizeof(RdsSym), false);
-    }
+    if (c.demod == B200_DEMOD_WFM_RDS_BITS) { return add_rds_demod(fe, v, v->chain.max_out(fe->max_eff)); }
     return 0;
 }
 
 // what one chunk of `count` samples can put into a VFO's output buffer, in 8-byte elements
-static int vfo_out_bound(const VfoSlot* v, int count) {
+static int vfo_out_bound(const b200_fe* fe, const VfoSlot* v, int count) {
+    if (is_rds_out(v)) {
+        // the parent's stages up to its discriminator (the IF blocks are 1:1), then the branch
+        const Chain& p = fe->vfos[v->rds_parent]->chain;
+        int n = count;
+        for (int i = 0; i <= p.quad_index(); i++) { n = p.st[i]->max_out(n); }
+        return b200_rds_demod_max_out(v->chain.max_out(n));
+    }
     int n = v->chain.max_out(count);
     // the high-pass FIR is 1:1 but its bound has a spare output: whether b200_fe_set_vfo_config switched it on or off since, the
     // bound stays the one b200_fe_add_vfo gave
@@ -598,7 +615,79 @@ static VfoSlot* get_slot(b200_fe* fe, int id) {
 static VfoSlot* get_vfo(b200_fe* fe, int id) {
     VfoSlot* v = get_slot(fe, id);
     if (v && is_tap(v)) { set_error("id %d is an IQ tap, not a VFO", id); return nullptr; }
+    if (v && is_rds_out(v)) { set_error("id %d is the RDS output of VFO %d, not a VFO", id, v->rds_parent); return nullptr; }
     return v;
+}
+static int new_slot_id(b200_fe* fe) {
+    for (size_t i = 0; i < fe->vfos.size(); i++) {
+        if (!fe->vfos[i]->used) { return (int)i; }
+    }
+    if (fe->vfos.size() >= B200_MAX_VFOS) { return -1; }
+    fe->vfos.push_back(std::make_unique<VfoSlot>());
+    return (int)fe->vfos.size() - 1;
+}
+
+// BroadcastFM::setRDSOut calls reset() (broadcast_fm.h:121-142): the discriminator's previous sample, the stereo stage (pilot
+// filter, PLL, delays) and the 15 kHz low-pass restart; RxVFO, the IF chain and the AF chain keep their state.  Device idle.
+static void restart_broadcast_fm(VfoSlot* p) {
+    Chain& ch = p->chain;
+    const int q = ch.quad_index();
+    const int n = (p->cfg.demod == B200_DEMOD_WFM_STEREO && p->cfg.low_pass) ? 3 : 2;     // QUAD, FIRR / M2S / STEREO [, FIRC]
+    for (int i = q; i < q + n && i < (int)ch.st.size(); i++) { clear_stage_state(*ch.st[i]); }
+    cudaDeviceSynchronize();          // legacy-stream memsets: done before the library's streams go on
+}
+
+// BroadcastFM's rdsOut (broadcast_fm.h:165-170,196-202) on a WFM VFO: the branch behind its own discriminator, RDSDemod behind it
+extern "C" int b200_fe_bind_rds(b200_fe* fe, int vfo_id) {
+    if (!fe) { set_error("null fe"); return B200_EINVAL; }
+    std::lock_guard<std::mutex> lck(fe->mtx);
+    VfoSlot* p = get_vfo(fe, vfo_id);
+    if (!p) { return B200_EINVAL; }
+    if (p->cfg.demod != B200_DEMOD_WFM && p->cfg.demod != B200_DEMOD_WFM_STEREO) {
+        set_error("VFO %d: RDS binds to a B200_DEMOD_WFM or B200_DEMOD_WFM_STEREO VFO", vfo_id);
+        return B200_EINVAL;
+    }
+    if (p->rds_child >= 0) { set_error("VFO %d already has an RDS output (id %d)", vfo_id, p->rds_child); return B200_EINVAL; }
+    B200_CK(cudaDeviceSynchronize());
+    const int id = new_slot_id(fe);
+    if (id < 0) { set_error("too many VFOs, IQ taps and RDS outputs"); return B200_ECAP; }
+    QuadStage* q = (QuadStage*)p->chain.st[p->chain.quad_index()].get();
+    if (p->rds_parked) {
+        // the branch resumes where the unbind left it: the reference's xlator, rdsResamp and rdsDemod are not reset by the toggle
+        fe->vfos[id] = std::move(p->rds_parked);
+    }
+    else {
+        auto b = std::make_unique<VfoSlot>();
+        int n_max = fe->max_eff;
+        for (int i = 0; i <= p->chain.quad_index(); i++) { n_max = p->chain.st[i]->max_out(n_max); }
+        int rc = b->chain.add_rds_branch(p->cfg.out_samplerate);
+        if (!rc) { rc = b->chain.finalize(n_max); }
+        if (!rc) { rc = add_rds_demod(fe, b.get(), b->chain.max_out(n_max)); }
+        if (rc) { return rc; }
+        b->chain.parent = &p->chain;
+        b->rds_parent = vfo_id;
+        b->used = true;
+        fe->vfos[id] = std::move(b);
+    }
+    q->side = (RxlStage*)fe->vfos[id]->chain.st[0].get();
+    p->rds_child = id;
+    restart_broadcast_fm(p);
+    return id;
+}
+extern "C" int b200_fe_unbind_rds(b200_fe* fe, int id) {
+    if (!fe) { set_error("null fe"); return B200_EINVAL; }
+    std::lock_guard<std::mutex> lck(fe->mtx);
+    VfoSlot* v = get_slot(fe, id);
+    if (!v) { return B200_EINVAL; }
+    if (!is_rds_out(v)) { set_error("id %d is not an RDS output", id); return B200_EINVAL; }
+    B200_CK(cudaDeviceSynchronize());
+    VfoSlot* p = fe->vfos[v->rds_parent].get();
+    ((QuadStage*)p->chain.st[p->chain.quad_index()].get())->side = nullptr;
+    p->rds_child = -1;
+    p->rds_parked = std::move(fe->vfos[id]);          // parked with its state, as chain::setBlockEnabled keeps a disabled block
+    fe->vfos[id] = std::make_unique<VfoSlot>();
+    restart_broadcast_fm(p);
+    return 0;
 }
 
 // IQFrontEnd::bindIQStream / unbindIQStream (iq_frontend.h:34-35): an id of the VFO id space, no state of its own
@@ -648,7 +737,9 @@ extern "C" int b200_fe_unbind_iq(b200_fe* fe, int id) {
 extern "C" int b200_fe_remove_vfo(b200_fe* fe, int id) {
     if (!fe) { set_error("null fe"); return B200_EINVAL; }
     std::lock_guard<std::mutex> lck(fe->mtx);
-    if (!get_vfo(fe, id)) { return B200_EINVAL; }
+    VfoSlot* v = get_vfo(fe, id);
+    if (!v) { return B200_EINVAL; }
+    if (v->rds_child >= 0) { set_error("VFO %d has an RDS output (id %d): unbind it first", id, v->rds_child); return B200_ESTATE; }
     B200_CK(cudaDeviceSynchronize());
     fe->vfos[id] = std::make_unique<VfoSlot>();
     return 0;
@@ -710,7 +801,7 @@ extern "C" int b200_fe_vfo_max_out(b200_fe* fe, int id, int count) {
     VfoSlot* v = get_slot(fe, id);
     if (!v) { return B200_EINVAL; }
     if (is_tap(v)) { return std::max(count, 0); }      // one sample per sample of the effective stream
-    return vfo_out_bound(v, count);
+    return vfo_out_bound(fe, v, count);
 }
 extern "C" int b200_fe_fft_max_lines(b200_fe* fe, int count) {
     if (!fe || !fe->fft_on) { return 0; }
@@ -810,6 +901,11 @@ extern "C" int b200_fe_reset(b200_fe* fe) {
         if (v->used && !is_tap(v.get())) { v->chain.reset_state(); }     // a tap has no state: it reads what the reset below clears
         if (v->used && v->rds) { int rcr = v->rds->reset(nullptr); if (rcr) { return rcr; } }
         for (auto& p : v->parked) { if (p) { clear_stage_state(*p); } }     // a block switched on later starts fresh
+        if (v->rds_parked) {                                                 // so does an RDS branch bound again later
+            v->rds_parked->chain.reset_state();
+            int rcr = v->rds_parked->rds->reset(nullptr);
+            if (rcr) { return rcr; }
+        }
     }
     B200_CK(cudaDeviceSynchronize());
     int rc = fe->sch.reset_raw();
@@ -1130,15 +1226,18 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
     std::vector<Chain*> chains;
     std::vector<int> ids, taps;
     for (size_t i = 0; i < fe->vfos.size(); i++) {
-        if (!fe->vfos[i]->used) { continue; }
-        if (is_tap(fe->vfos[i].get())) { taps.push_back((int)i); }
-        else { chains.push_back(&fe->vfos[i]->chain); ids.push_back((int)i); }
+        const VfoSlot* v = fe->vfos[i].get();
+        if (!v->used || is_rds_out(v)) { continue; }
+        if (is_tap(v)) { taps.push_back((int)i); continue; }
+        chains.push_back(&fe->vfos[i]->chain); ids.push_back((int)i);
+        // a bound RDS branch right behind the VFO whose discriminator feeds it (Chain::parent)
+        if (v->rds_child >= 0) { chains.push_back(&fe->vfos[v->rds_child]->chain); ids.push_back(v->rds_child); }
     }
     // samples that reach the FFT branch and the VFOs: the chunk itself, or what the input decimator makes of it
     const int ecount = (fe->decim > 1) ? fe->pre.peek(count) : count;
     if (ecount < 0) { set_error("input decimator is not a FIR cascade"); return B200_ESTATE; }
     for (size_t k = 0; k < chains.size(); k++) {
-        int bound = vfo_out_bound(fe->vfos[ids[k]].get(), ecount);
+        int bound = vfo_out_bound(fe, fe->vfos[ids[k]].get(), ecount);
         if (out->vfo_out[ids[k]] == nullptr || out->vfo_cap[ids[k]] < bound) {
             set_error("VFO %d output buffer too small: need room for %d samples (b200_fe_vfo_max_out)", ids[k], bound);
             return B200_ECAP;
@@ -1227,7 +1326,7 @@ extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt
         in_fmt = cur_fmt;
         count = ecount;
     }
-    for (Chain* c : chains) { c->plan(count); }
+    for (Chain* c : chains) { c->plan(c->parent ? c->parent->st[c->parent->quad_index()]->n_out : count); }
     // device-resident outputs: the last stage of every chain (and the FFT epilogue) write straight into the caller's buffers
     const bool direct = (out->out_mem == B200_MEM_DEVICE);
     // host outputs of a small chunk: the last kernel of a VFO stores straight into the caller's pinned buffer (a few KB over

@@ -593,6 +593,10 @@ int Chain::plan(int n) {
     n_out = n;
     return n;
 }
+int Chain::quad_index() const {
+    for (size_t i = 0; i < st.size(); i++) { if (st[i]->kind == K_QUAD) { return (int)i; } }
+    return -1;
+}
 int Chain::max_out(int n) const {
     for (auto& s : st) { n = s->max_out(n); }
     return n;
@@ -771,6 +775,9 @@ int Chain::add_wfm(double deviationHz, double samplerate, bool lowPass, bool ste
 int Chain::add_wfm_rds(double deviationHz, double samplerate) {
     int rc = add_quad(deviationHz, samplerate);
     if (rc) { return rc; }
+    return add_rds_branch(samplerate);
+}
+int Chain::add_rds_branch(double samplerate) {
     auto x = std::make_unique<RxlStage>();
     x->set_offset_rad(hz_to_rads(-57000.0, samplerate));                 // xlator.init(NULL, -57000.0, samplerate)
     st.push_back(std::move(x));
@@ -1155,8 +1162,10 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
         B200_CK(cudaStreamWaitEvent(stream, ev_tail[parity], 0));
     }
     trace_mark("stage1 start", stream);
+    // level of a chain's first stage in the level-by-level section: an RDS branch starts at its parent's discriminator
+    auto lvl0 = [](const Chain* c) -> size_t { return c->parent ? (size_t)std::max(0, c->parent->quad_index()) : 0; };
     for (Chain* c : chains) {
-        depth = std::max(depth, c->st.size());
+        depth = std::max(depth, lvl0(c) + c->st.size());
         for (size_t i = 0; i < c->st.size(); i++) {
             Stage* s = c->st[i].get();
             s->out_ptr = (i + 1 < c->st.size()) ? c->st[i + 1]->in_data() : (c->out_override ? c->out_override : c->out.as<float>());
@@ -1489,6 +1498,7 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
                 J.nat_off = c->fp.nat_off;
                 J.stg_floats = c->fp.stg2_rel;
                 J.taps_nat = c->fp.s0_direct ? ((FirCStage*)c->st[c->fp.beg].get())->taps.as<float>() : nullptr;
+                J.rds = nullptr; J.rds_phase0 = 0; J.rds_w = 0;
                 for (int i = 0; i < nst; i++) {
                     Stage* sg = c->st[c->fp.beg + i].get();
                     FtStage& d = J.st[i];
@@ -1497,6 +1507,10 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
                     d.buf = c->fp.buf[i]; d.pitch = c->fp.pitch[i]; d.tap_off = c->fp.tap_off[i]; d.qpitch = c->fp.qpitch[i];
                     if (sg->kind == K_FIRC) { d.off = ((FirCStage*)sg)->chunk_offset; }
                     if (sg->kind == K_POLY) { d.off = ((PolyStage*)sg)->chunk_offset; d.phase = ((PolyStage*)sg)->chunk_phase; }
+                    if (sg->kind == K_QUAD && ((QuadStage*)sg)->side) {
+                        const RxlStage* x = ((QuadStage*)sg)->side;
+                        J.rds = (float2*)x->out_ptr; J.rds_phase0 = x->chunk_phase0; J.rds_w = x->w;
+                    }
                     if (i > 0) {
                         d.hist_rd = sg->fh[sg->fpar].as<float>();
                         d.hist_wr = sg->fh[sg->fpar ^ 1].as<float>();
@@ -1555,9 +1569,10 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
             return 0;
         };
         for (Chain* c : chains) {
-            if (lvl >= c->st.size()) { continue; }
+            const size_t l0 = lvl0(c);
+            if (lvl < l0 || lvl - l0 >= c->st.size()) { continue; }
             if (c->fp.active && lvl >= 1 && (int)lvl < c->fp.end) { continue; }     // done by the fused launch
-            Stage* s = c->st[lvl].get();
+            Stage* s = c->st[lvl - l0].get();
             int rc = 0;
             switch (s->kind) {
             case K_XD: break;
@@ -1608,6 +1623,8 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
                 QuadJob& j = qp.job[qp.njobs++];
                 j.in = (const float2*)f->base(); j.out = f->out_ptr;
                 j.inv_dev = f->inv_dev; j.n = f->n_out;
+                j.rds = f->side ? (float2*)f->side->out_ptr : nullptr;
+                j.rds_phase0 = f->side ? f->side->chunk_phase0 : 0; j.rds_w = f->side ? f->side->w : 0;
                 qp.max_n = std::max(qp.max_n, f->n_out);
                 if (qp.njobs == B200_BATCH) { rc = flush_batch(qp, launch_quad, ts, launches); qp.max_n = 0; }
                 break;
@@ -1660,7 +1677,7 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
             }
             case K_RXL: {
                 RxlStage* f = (RxlStage*)s;
-                if (f->n_out <= 0) { break; }
+                if (f->n_out <= 0 || (c->parent && lvl == l0)) { break; }      // an RDS branch's: its parent's discriminator stored it
                 RxlJob& j = xlp.job[xlp.njobs++];
                 j.in = f->in_data(); j.out = (float2*)f->out_ptr; j.n = f->n_out; j.phase0 = f->chunk_phase0; j.w = f->w;
                 xlp.max_n = std::max(xlp.max_n, f->n_out);
@@ -1749,7 +1766,8 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
         if (rcs) { return rcs; }
     }
     else {
-        const size_t half = (all_chains.size() + 1) / 2;
+        size_t half = (all_chains.size() + 1) / 2;
+        while (half < all_chains.size() && all_chains[half]->parent) { half++; }     // an RDS branch stays with its parent
         std::vector<Chain*> ga(all_chains.begin(), all_chains.begin() + half), gb(all_chains.begin() + half, all_chains.end());
         rec.cur_branch = 0;
         int rcs = tail_section(ga);

@@ -129,8 +129,10 @@ struct PolyStage : Stage {
     void reset_state() override { phase = 0; offset = 0; }
 };
 
+struct RxlStage;
 struct QuadStage : Stage {
     float inv_dev = 1.0f;
+    RxlStage* side = nullptr;    // first stage of a bound RDS branch (b200_fe_bind_rds): this discriminator computes its output
     QuadStage() { kind = K_QUAD; out_es = 1; hist = 1; }   // history = the previous chunk's last sample (Quadrature::phase)
     int configure(double deviationHz, double samplerate);
     int plan(int n) override { n_in = n; n_out = n; return n; }
@@ -240,6 +242,11 @@ struct Chain {
     int n_out = 0;               // this chunk
     float* out_override = nullptr;   // this chunk: final stage writes straight into the caller's device buffer
     bool raw_input() const { return !st.empty() && st[0]->kind == K_XD; }
+    // an RDS branch bound to a WFM VFO (b200_fe_bind_rds): `parent`'s discriminator writes what st[0] (RxlStage) would, so
+    // st[0] launches nothing and st[i] runs at level quad_index() + i of the parent.  The scheduler takes the branch right
+    // behind its parent in the chain list.
+    const Chain* parent = nullptr;
+    int quad_index() const;      // index of the discriminator stage, -1 when there is none
     int chan_fir = -1;           // stage index of RxVFO's channel filter (rx_vfo.h:28-31), set by add_rxvfo
     FusedPlan fp;
     FuseCfg fcfg;
@@ -273,6 +280,7 @@ struct Chain {
     int add_af_chain(double afSamplerate, double audioSamplerate, bool highPass, double deemphTau);
     int add_af_highpass(double audioSamplerate);                            // taps::highPass(300, 100, audioSR) (radio_module.h:597-598)
     int add_wfm_rds(double deviationHz, double samplerate);                 // BroadcastFM's RDS branch: discriminator -> -57 kHz -> 5 kS/s (broadcast_fm.h:52-53,165-170)
+    int add_rds_branch(double samplerate);                                  // the part behind the discriminator: -57 kHz -> 5 kS/s
     int add_noise_blanker(double rate, double level);                       // noise_reduction::NoiseBlanker (noise_blanker.h:12-17)
     int add_fmif(int bins);                                                 // noise_reduction::FMIF (fm_if.h:20-24)
     int add_squelch(double level);                                          // noise_reduction::PowerSquelch (power_squelch.h:16-20)

@@ -461,6 +461,7 @@ __global__ void __launch_bounds__(NT, 2) k_tail_fused(const __grid_constant__ Ft
             }
             case FT_QUAD: {
                 const float2* X = reinterpret_cast<const float2*>(xb);
+                const int own_lo = J.rds ? ft_own_lo(J, slab, s) : 0, own_hi = J.rds ? ft_own_lo(J, slab + 1, s) : 0;
                 for (int base = t0; base < t1; base += NT) {
                     const int m = base + tid;
                     const bool act = m < t1;
@@ -475,7 +476,9 @@ __global__ void __launch_bounds__(NT, 2) k_tail_fused(const __grid_constant__ Ft
                         float diff = __fsub_rn(cur, prev);
                         if (diff > FL_M_PI_REF) { diff = __fsub_rn(diff, 2.0f * FL_M_PI_REF); }
                         else if (diff <= -FL_M_PI_REF) { diff = __fadd_rn(diff, 2.0f * FL_M_PI_REF); }
-                        dst.put1(m, __fmul_rn(diff, S.scale));
+                        const float v = __fmul_rn(diff, S.scale);
+                        dst.put1(m, v);
+                        if (m >= own_lo && m < own_hi) { J.rds[m] = rds_xlate(v, J.rds_phase0, J.rds_w, m); }
                     }
                 }
                 break;

@@ -65,6 +65,13 @@ __device__ __forceinline__ float2 phasor_u64(unsigned long long phase) {
     return make_float2(c, s);
 }
 
+// RealToComplex + FrequencyXlator of BroadcastFM's RDS branch (broadcast_fm.h:165-170) for sample i of a chunk whose first
+// sample has phase phase0: k_rxl, and the discriminators that feed a bound RDS output (k_quad, k_tail_fused), store exactly this
+__device__ __forceinline__ float2 rds_xlate(float v, unsigned long long phase0, unsigned long long w, int i) {
+    const float2 ph = phasor_u64(phase0 + w * (unsigned long long)i);
+    return make_float2(v * ph.x, v * ph.y);
+}
+
 __device__ __forceinline__ float2 cmulf(float2 a, float2 b) {
     return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
 }
@@ -229,7 +236,9 @@ __global__ void __launch_bounds__(256) k_quad(const __grid_constant__ QuadParams
     float diff = __fsub_rn(cur, prev);
     if (diff > FL_M_PI_REF) { diff = __fsub_rn(diff, 2.0f * FL_M_PI_REF); }
     else if (diff <= -FL_M_PI_REF) { diff = __fadd_rn(diff, 2.0f * FL_M_PI_REF); }
-    J.out[i] = __fmul_rn(diff, J.inv_dev);
+    const float v = __fmul_rn(diff, J.inv_dev);
+    J.out[i] = v;
+    if (J.rds) { J.rds[i] = rds_xlate(v, J.rds_phase0, J.rds_w, i); }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -266,9 +275,7 @@ __global__ void __launch_bounds__(256) k_rxl(const __grid_constant__ RxlParams p
     const RxlJob& J = p.job[blockIdx.y];
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= J.n) { return; }
-    const float v = __ldg(J.in + i);
-    const float2 ph = phasor_u64(J.phase0 + J.w * (unsigned long long)i);
-    J.out[i] = make_float2(v * ph.x, v * ph.y);
+    J.out[i] = rds_xlate(__ldg(J.in + i), J.phase0, J.w, i);
 }
 
 // ------------------------------------------------------------------------------------------------

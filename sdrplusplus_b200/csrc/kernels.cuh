@@ -108,6 +108,9 @@ struct QuadJob {
     float* out;
     float inv_dev;
     int n;
+    // a bound RDS output (b200_fe_bind_rds): rds[i] = the branch's translated multiplex (rds_xlate), else null
+    float2* rds;
+    unsigned long long rds_phase0, rds_w;
 };
 struct QuadParams { int njobs; int max_n; QuadJob job[B200_BATCH]; };
 
@@ -163,6 +166,10 @@ struct FtJob {
     const float* taps_nat;
     const float* src;           // stage 0 input: [hist | data] in global memory
     float* out;                 // final output
+    // the FT_QUAD stage of a VFO with a bound RDS output also stores its branch input (QuadJob::rds), each sample once: a slab
+    // stores the discriminator outputs it owns (ft_own_lo), not the halo it recomputes for its neighbour
+    float2* rds;
+    unsigned long long rds_phase0, rds_w;
     FtStage st[FT_MAXST];
 };
 struct FtParams { int njobs; int pad; long long* dbg; FtJob job[B200_BATCH]; };   // dbg: optional per-stage clock64() of CTA (1,0)
@@ -216,6 +223,21 @@ FT_HD inline void ft_ranges(const FtJob& J, int slab, int* lo, int* hi) {
         }
         lo[s] = ilo; hi[s] = ihi;
     }
+}
+// first output of stage s that slab `slab` owns: where the input range of the stage behind it starts for the slab's first final
+// output, before the last slab's history extension (ft_ranges).  Slab k owns [ft_own_lo(k), ft_own_lo(k + 1)), the last slab
+// up to n_out: the slabs partition the stage's outputs, and each owns only outputs it computes.
+FT_HD inline int ft_own_lo(const FtJob& J, int slab, int s) {
+    const int n = J.st[s].n_out;
+    if (slab <= 0) { return 0; }
+    if (slab >= J.slabs) { return n; }
+    int m = slab * J.OB;
+    for (int k = J.nst - 1; k > s; k--) {
+        int ilo, ihi;
+        ft_need_in(J.st[k], m > 0 ? m : 0, (m > 0 ? m : 0) + 1, ilo, ihi);
+        m = ilo;
+    }
+    return m < 0 ? 0 : (m > n ? n : m);
 }
 cudaError_t launch_tail_fused(const FtParams& p, int max_slabs, int threads, size_t smem_bytes, cudaStream_t s);
 int tail_fused_ctas_per_sm(int threads, size_t smem_bytes);

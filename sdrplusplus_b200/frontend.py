@@ -140,6 +140,7 @@ class FrontEnd:
         self.fft_size = 0
         self.vfos = {}
         self.taps = {}               # IQ tap id -> sample type
+        self.rds = {}                # RDS output id -> the WFM VFO it is bound to
 
     def close(self):
         if getattr(self, "_h", None):
@@ -191,6 +192,17 @@ class FrontEnd:
         L.check(self._l.b200_fe_unbind_iq(self._h, tid))
         self.taps.pop(tid, None)
 
+    def bind_rds(self, vid):
+        """The radio's "Decode RDS" on WFM VFO `vid`: BroadcastFM's RDS branch off that VFO's own discriminator, its symbols
+        delivered by every later process() under the returned id as a DEMOD_WFM_RDS_BITS VFO's (b200_fe_bind_rds)."""
+        rid = L.check(self._l.b200_fe_bind_rds(self._h, int(vid)))
+        self.rds[rid] = int(vid)
+        return rid
+
+    def unbind_rds(self, rid):
+        L.check(self._l.b200_fe_unbind_rds(self._h, rid))
+        self.rds.pop(rid, None)
+
     def set_vfo_offset(self, vid, offset):
         L.check(self._l.b200_fe_set_vfo_offset(self._h, vid, float(offset)))
 
@@ -240,7 +252,7 @@ class FrontEnd:
     def _alloc_outputs(self, count):
         o = L.Outputs()
         bufs = {}
-        for vid, cfg in self.vfos.items():
+        for vid in list(self.vfos) + list(self.rds):
             cap = self.vfo_max_out(vid, count)
             b = np.empty(cap * 2, np.float32)
             bufs[vid] = b
@@ -262,8 +274,8 @@ class FrontEnd:
         return o, bufs, fft
 
     def process(self, iq, fmt=L.FMT_CF32):
-        """Host numpy in, host numpy out.  Returns ({vfo_id: array}, fft_lines[n, N]); a DEMOD_WFM_RDS_BITS VFO gives the
-        pair (soft float32, bit uint8), an IQ tap complex64 (IQ_CF32) or (n, 2) uint8 / int8 / int16 / int32."""
+        """Host numpy in, host numpy out.  Returns ({vfo_id: array}, fft_lines[n, N]); a DEMOD_WFM_RDS_BITS VFO and an RDS
+        output (bind_rds) give the pair (soft float32, bit uint8), an IQ tap complex64 (IQ_CF32) or (n, 2) uint8 / int8 / int16 / int32."""
         a, count = _as_input(iq, fmt)
         o, bufs, fft = self._alloc_outputs(count)
         L.check(self._l.b200_fe_process(self._h, a.ctypes.data, count, fmt, L.MEM_HOST, C.byref(o)))
@@ -277,13 +289,15 @@ class FrontEnd:
             outs[vid] = y.view(np.complex64) if cfg.demod in (L.DEMOD_RAW, L.DEMOD_WFM_RDS) else y.reshape(-1, 2)
         for tid in self.taps:
             outs[tid] = bufs[tid][: o.vfo_count[tid]].copy()
+        for rid in self.rds:
+            outs[rid] = rds_symbols(bufs[rid], o.vfo_count[rid])
         lines = fft[: o.fft_lines].copy() if fft is not None else np.empty((0, 0), np.float32)
         return outs, lines
 
     def process_chunks(self, iq, chunk, fmt=L.FMT_CF32):
         a, count = _as_input(iq, fmt)
         per = _NP_FMT[fmt][1]
-        acc = {vid: [] for vid in list(self.vfos) + list(self.taps)}
+        acc = {vid: [] for vid in list(self.vfos) + list(self.taps) + list(self.rds)}
         lines = []
         for i in range(0, count, chunk):
             outs, ln = self.process(a[i * per:(i + chunk) * per], fmt)
@@ -295,7 +309,7 @@ class FrontEnd:
         for vid, v in acc.items():
             if vid in self.taps:
                 res[vid] = np.concatenate(v) if v else iq_tap_array(self.taps[vid], 0)
-            elif self.vfos[vid].demod == L.DEMOD_WFM_RDS_BITS:
+            elif vid in self.rds or self.vfos[vid].demod == L.DEMOD_WFM_RDS_BITS:
                 res[vid] = (np.concatenate([p[0] for p in v]) if v else np.empty(0, np.float32),
                             np.concatenate([p[1] for p in v]) if v else np.empty(0, np.uint8))
             else:

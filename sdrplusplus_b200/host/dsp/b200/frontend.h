@@ -48,10 +48,36 @@ namespace dsp::b200 {
         void removeVFO(int id) {
             std::lock_guard<std::recursive_mutex> lk(ctrlMtx);
             tempStop();
-            if (b200_fe_remove_vfo(fe, id) == 0 && id < (int)outs_.size() && outs_[id]) {
-                unregisterOutput(outs_[id]);
-                delete outs_[id];
-                outs_[id] = nullptr;
+            for (size_t i = 0; i < rds_.size(); i++) {
+                if (rds_[i].vfo == id) { unbindRDS(rds_[i].id); break; }
+            }
+            if (b200_fe_remove_vfo(fe, id) == 0) { dropOut(id); }
+            tempStart();
+        }
+        // the radio's "Decode RDS" (BroadcastFM::setRDSOut, demodulators/wfm.h:118-119) on a WFM VFO: returns an id whose
+        // stream, vfoOut(id), carries one b200_rds_symbol per recovered symbol (read them with rdsSymbols), decoded from that
+        // VFO's own discriminator beside its audio (b200_fe_bind_rds)
+        int bindRDS(int vfoId) {
+            std::lock_guard<std::recursive_mutex> lk(ctrlMtx);
+            tempStop();
+            int id = b200_fe_bind_rds(fe, vfoId);
+            if (id >= 0) {
+                if ((int)outs_.size() <= id) { outs_.resize(id + 1, nullptr); }
+                outs_[id] = new stream<stereo_t>(b200_fe_vfo_max_out(fe, id, _in->bufferSize()));
+                registerOutput(outs_[id]);
+                rds_.push_back({ vfoId, id });
+            }
+            tempStart();
+            return id;
+        }
+        void unbindRDS(int id) {
+            std::lock_guard<std::recursive_mutex> lk(ctrlMtx);
+            tempStop();
+            if (b200_fe_unbind_rds(fe, id) == 0) {
+                dropOut(id);
+                for (size_t i = 0; i < rds_.size(); i++) {
+                    if (rds_[i].id == id) { rds_.erase(rds_.begin() + i); break; }
+                }
             }
             tempStart();
         }
@@ -134,6 +160,13 @@ namespace dsp::b200 {
             return count;
         }
     private:
+        void dropOut(int id) {
+            if (id < (int)outs_.size() && outs_[id]) {
+                unregisterOutput(outs_[id]);
+                delete outs_[id];
+                outs_[id] = nullptr;
+            }
+        }
         void updateFFTPath() {
             std::lock_guard<std::recursive_mutex> lk(ctrlMtx);
             tempStop();
@@ -149,6 +182,8 @@ namespace dsp::b200 {
         std::vector<stream<stereo_t>*> outs_;
         struct BoundIQ { stream<complex_t>* s; int id; };
         std::vector<BoundIQ> iqs_;
+        struct BoundRDS { int vfo, id; };
+        std::vector<BoundRDS> rds_;
         float* lines = nullptr;
         int size = 0;
         float* (*acquire)(void*) = nullptr;

@@ -77,6 +77,8 @@ SIGNATURES = {
     "b200_fe_set_vfo_config": (_i, [_vp, _i, C.POINTER(VfoCfg)]),
     "b200_fe_bind_iq": (_i, [_vp, _i, C.c_float]),
     "b200_fe_unbind_iq": (_i, [_vp, _i]),
+    "b200_fe_bind_rds": (_i, [_vp, _i]),
+    "b200_fe_unbind_rds": (_i, [_vp, _i]),
     "b200_fe_vfo_count": (_i, [_vp]),
     "b200_fe_vfo_max_out": (_i, [_vp, _i, _i]),
     "b200_fe_fft_max_lines": (_i, [_vp, _i]),

@@ -1,14 +1,16 @@
 """RDS for every station of a band: step time of a 100 MS/s stream with 8 WFM VFOs and RDS symbols for the same 8 stations,
 decoded either inside the front end (8 B200_DEMOD_WFM_RDS_BITS VFOs, one RDSDemod launch per chunk on the tail stream) or
 by the two-piece path (8 B200_DEMOD_WFM_RDS VFOs whose 5 kS/s streams go to 8 stand-alone b200_rds_demod handles after every
-wait).  A third leg, 8 WFM + 8 WFM_RDS with no symbol decoding at all, is the floor both are compared with.
+wait).  A third leg, 8 WFM + 8 WFM_RDS with no symbol decoding at all, is the floor both are compared with.  The leg "bound"
+decodes the same symbols from the 8 WFM VFOs' own discriminators (b200_fe_bind_rds, the radio's "Decode RDS"), and
+"wfm_only" runs the 8 WFM VFOs alone.  --parent stereo makes every leg's WFM VFOs B200_DEMOD_WFM_STEREO.
 
 Every leg pipelines submit / wait with two chunks in flight on a device-resident input, outputs in pinned b200_host_alloc
 buffers, and the legs alternate (--rounds) so that drift of the shared machine shows up as spread, not as a difference.
 Prints one JSON line: per leg the mean step time (ms) of each round, the symbols recovered per second of wall time and the
 5 kS/s samples per second they came from, with the card's name and power limit read in the same run.
 
-    python tools/rds_band_step.py --steps 40 --warmup 5 [--chunk 16777216] [--rounds 3]
+    python tools/rds_band_step.py --steps 40 --warmup 5 [--chunk 16777216] [--rounds 3] [--parent stereo] [--legs bound,bits,wfm_only]
 """
 import argparse
 import ctypes as C
@@ -59,11 +61,17 @@ def make_input(chunk, nbuf):
     return torch.view_as_real(x).contiguous()
 
 
-def leg(sb, lib, L, xin, chunk, nbuf, mode, steps, warmup):
-    """mode: "bits" (RDSDemod in the front end), "two_piece" (stand-alone handles), "none" (5 kS/s streams, no decoding)"""
+def leg(sb, lib, L, xin, chunk, nbuf, mode, steps, warmup, parent="mono"):
+    """mode: "bits" (RDSDemod in the front end), "two_piece" (stand-alone handles), "none" (5 kS/s streams, no decoding),
+    "bound" (RDS bound to the WFM VFOs), "wfm_only" (no RDS)"""
     fe = sb.FrontEnd(FS, chunk)
-    wfm = [fe.add_vfo(sb.VfoConfig.wfm(o)) for o in OFFS]
-    side = [fe.add_vfo(sb.VfoConfig.wfm_rds_bits(o) if mode == "bits" else sb.VfoConfig.wfm_rds(o)) for o in OFFS]
+    wfm = [fe.add_vfo((sb.VfoConfig.wfm_stereo if parent == "stereo" else sb.VfoConfig.wfm)(o)) for o in OFFS]
+    if mode == "bound":
+        side = [fe.bind_rds(v) for v in wfm]
+    elif mode == "wfm_only":
+        side = []
+    else:
+        side = [fe.add_vfo(sb.VfoConfig.wfm_rds_bits(o) if mode == "bits" else sb.VfoConfig.wfm_rds(o)) for o in OFFS]
     demods = [sb.RdsDemod() for _ in OFFS] if mode == "two_piece" else []
     outs, bufs = [], []
     for _ in range(2):
@@ -84,10 +92,10 @@ def leg(sb, lib, L, xin, chunk, nbuf, mode, steps, warmup):
                 y = np.ctypeslib.as_array((C.c_float * (2 * n)).from_address(o.vfo_out[v])).view(np.complex64) if n else np.empty(0, np.complex64)
                 nsym = demods[j].process(y)[0].size
             else:
-                nsym = n if mode == "bits" else 0
+                nsym = n if mode in ("bits", "bound") else 0
             if timed:
                 stats["symbols"] += nsym
-                stats["rds_in"] += n if mode != "bits" else 0     # the 5 kS/s count of a bits VFO is not an output
+                stats["rds_in"] += n if mode not in ("bits", "bound") else 0     # the 5 kS/s count of a bits VFO is not an output
     base = xin.data_ptr()
     total = steps + warmup
     pend, t0, timed = [], None, 0
@@ -122,6 +130,8 @@ def main():
     ap.add_argument("--chunk", type=int, default=1 << 24)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--nbuf", type=int, default=3)
+    ap.add_argument("--parent", choices=("mono", "stereo"), default="mono")
+    ap.add_argument("--legs", default="bits,two_piece,none")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -133,19 +143,21 @@ def main():
     L.b200_init(0)
     ident = card()
     xin = make_input(a.chunk, a.nbuf)
-    res = {m: {"step_ms": [], "symbols_per_s": [], "rds_5ksps_per_s": []} for m in ("bits", "two_piece", "none")}
+    res = {m: {"step_ms": [], "symbols_per_s": [], "rds_5ksps_per_s": []} for m in a.legs.split(",")}
     for _ in range(a.rounds):
         for m in res:
-            ms, sps, ins = leg(sb, lib, L, xin, a.chunk, a.nbuf, m, a.steps, a.warmup)
+            ms, sps, ins = leg(sb, lib, L, xin, a.chunk, a.nbuf, m, a.steps, a.warmup, a.parent)
             res[m]["step_ms"].append(round(ms, 3))
             res[m]["symbols_per_s"].append(round(sps, 1))
             res[m]["rds_5ksps_per_s"].append(round(ins, 1))
     for m, r in res.items():
         r["step_ms_mean"] = round(float(np.mean(r["step_ms"])), 3)
-        if m == "bits":
+        r["step_ms_median"] = round(float(np.median(r["step_ms"])), 3)
+        r["step_ms_spread"] = round(float(np.max(r["step_ms"]) - np.min(r["step_ms"])), 3)
+        if m in ("bits", "bound"):
             del r["rds_5ksps_per_s"]          # the same chain as the other legs; its 5 kS/s stream never leaves the device
     print(json.dumps({"tool": "rds_band_step", "card": ident, "samplerate": FS, "chunk": a.chunk, "steps": a.steps,
-                      "warmup": a.warmup, "rounds": a.rounds, "vfos": {"wfm": 8, "rds": 8}, "legs": res}))
+                      "warmup": a.warmup, "rounds": a.rounds, "parent": a.parent, "vfos": {"wfm": 8, "rds": 8}, "legs": res}))
 
 
 if __name__ == "__main__":
