@@ -930,7 +930,7 @@ static cudaError_t launch_xd_tma_n(const XdParams& p, const XtGeom& g, const CUt
     // the epilogue).  At config 2 (8 VFOs, PS 10) that is 141.3 KiB: with a pass-1 FFT CTA of 8 (82.1 KiB) and 2 x 1 KiB
     // reserved it stays within the SM's 228 KiB
     auto bytes = [&](int nj, bool f2) {
-        return (size_t)NST * Lay::STAGE + ((size_t)nj * (PS + 16) + (size_t)Lay::NW * nj * 4 + (f2 ? (size_t)nj * Lay::F2H : 0)) * sizeof(float2) +
+        return (size_t)NST * Lay::STAGE + ((size_t)nj * (PS + 16 + Lay::NPH) + (f2 ? (size_t)nj * Lay::F2H : 0)) * sizeof(float2) +
                2 * NST * sizeof(unsigned long long) + 1024;
     };
     const size_t smem = bytes(p.njobs, g.f2 != 0);

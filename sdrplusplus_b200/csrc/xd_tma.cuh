@@ -11,10 +11,11 @@
 //     one tile = NSEG*2 boxes of {16 samples, NR super-rows} with the 128-byte swizzle, issued by ONE thread, landing in
 //     shared memory as [segment][block parity][row][128 B].  No thread touches the data on its way in.
 //   * a persistent CTA per SM runs a ring of XT_STAGES tiles guarded by full / empty mbarriers: a producer warp keeps
-//     two tiles in flight while MT/64 consumer warps filter the third, so HBM latency never reaches the FMAs.
-//   * a lane owns two ADJACENT outputs; their windows (QC+1 blocks) sit in consecutive rows of the two parity regions,
-//     so every 16-byte window load of a warp is conflict-free through the hardware swizzle and feeds four packed FMAs;
-//     the real taps come from the kernel parameter block (constant bank), not from shared memory.
+//     the next tile in flight while MT/32 consumer warps (two per SM scheduler at D = 32) filter the one that landed.
+//   * a lane owns ONE output and its window of QC blocks; a warp's 32 outputs are consecutive, lanes 0-15 take the even
+//     ones and lanes 16-31 the odd ones (xt_lane_out), so that the eight lanes of a quarter warp read eight consecutive
+//     rows of one parity region and every 16-byte window load is conflict-free through the hardware swizzle; a load feeds
+//     two packed FMAs.  The real taps come from the kernel parameter block (constant bank), not from shared memory.
 // Rows are cut at a 128-byte aligned origin org' <= org; the s = org - org' samples in front of a window are covered
 // by s leading zero taps: the accumulator class of window position p is p mod PS, the tap it carries is k = p - s.
 //
@@ -78,7 +79,8 @@ struct XtLay {
     static constexpr int NR = (NEED + 7) & ~7;                           // rows per region (whole swizzle atoms)
     static constexpr int REGION = NR * 128;
     static constexpr int STAGE = NSEG * 2 * REGION;
-    static constexpr int NW = MT / 64;                                   // consumer warps
+    static constexpr int NW = MT / 32;                                   // consumer warps, 32 outputs each
+    static constexpr int NPH = MT / 16;                                  // coarse phases per job and tile (one per 16 outputs)
     // ÷4 epilogue: per job, the 26 carried stage-1 outputs and the MT of the tile, staged in the ring slot the tile came in,
     // one pad entry per 16 (a thread reads the 39-entry window of four ÷4 outputs; neighbouring threads are 16 apart)
     static constexpr int F2H = XD_F2_T - 1;
@@ -87,33 +89,29 @@ struct XtLay {
     static_assert(MT % 16 == 0, "whole groups of four ÷4 outputs per tile");
 };
 __device__ __forceinline__ int xt_f2_pad(int i) { return i + (i >> 4); }
+// output of a consumer lane within its warp's 32: lanes 0-15 the even ones, lanes 16-31 the odd ones
+__device__ __forceinline__ int xt_lane_out(int lane) { return ((lane & 15) << 1) | (lane >> 4); }
 
 // decimation-phase pairs [RP0, RP1) of a tile -- they all lie in ONE 128-byte segment (8 pairs per segment), whose two parity
-// regions start at sb -- into the 2 x PS class sums of a lane.  Every index is a compile-time constant: taps from the constant
-// bank, accumulators in registers.
-template <int LOGD, int QC, int PS, int REGION, int RP0, int RP1, int NQH>
-__device__ __forceinline__ void xt_accumulate(float2 (&S)[2][PS], const XtGeom& g, unsigned sb, const unsigned (&aoff)[NQH]) {
+// regions start at sb -- into the PS class sums of a lane's output.  Every index is a compile-time constant: taps from the
+// constant bank, accumulators in registers.  aoff[q]: the offset of the row of window block q in its parity region's segment.
+template <int LOGD, int QC, int PS, int RP0, int RP1>
+__device__ __forceinline__ void xt_accumulate(float2 (&S)[PS], const XtGeom& g, unsigned sb, const unsigned (&aoff)[QC]) {
     constexpr int D = 1 << LOGD;
     static_assert((RP0 >> 3) == ((RP1 - 1) >> 3), "one segment per call");
 #pragma unroll
     for (int rp = RP0; rp < RP1; rp++) {
 #pragma unroll
-        for (int q = 0; q <= QC; q++) {
-            const unsigned addr = sb + (unsigned)((q & 1) * REGION) + (aoff[q >> 1] ^ (unsigned)((rp & 7) << 4));
+        for (int q = 0; q < QC; q++) {
+            const unsigned addr = (sb + aoff[q]) ^ (unsigned)((rp & 7) << 4);    // sb: 1024-byte aligned
             float4 x;
             asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];\n" : "=f"(x.x), "=f"(x.y), "=f"(x.z), "=f"(x.w) : "r"(addr));
 #pragma unroll
             for (int e = 0; e < 2; e++) {
                 const int r = 2 * rp + e;
                 const float2 xe = e ? make_float2(x.z, x.w) : make_float2(x.x, x.y);
-                if (q < QC) {
-                    const float t = g.g[q * D + r];
-                    S[0][(q * D + r) % PS] = ffma2(make_float2(t, t), xe, S[0][(q * D + r) % PS]);
-                }
-                if (q >= 1) {
-                    const float t = g.g[(q - 1) * D + r];
-                    S[1][((q - 1) * D + r) % PS] = ffma2(make_float2(t, t), xe, S[1][((q - 1) * D + r) % PS]);
-                }
+                const float t = g.g[q * D + r];
+                S[(q * D + r) % PS] = ffma2(make_float2(t, t), xe, S[(q * D + r) % PS]);
             }
         }
     }
@@ -122,12 +120,15 @@ __device__ __forceinline__ void xt_accumulate(float2 (&S)[2][PS], const XtGeom& 
 // What bounds it is measured by switching the filter or the loads off (option "s1_diag", tools/s1_bounds.py).  Three
 // restructurings of the consumer side are in the history (two groups of warps sharing a tile, ring slots of one 128-byte
 // segment, filter warps handing their class sums to combine warps); none was faster on the GPU they were measured on.
+// One output per lane (8 consumer warps instead of 4 at D = 32), on an H100 80GB HBM3 at 700 W: stage 1 alone 76.9 -> 68.7 us,
+// bench `value` 109.3 -> 113.6 GS/s (medians of three alternated runs), same output bits.
+// At most 96 registers per thread: at D = 32 the 288 threads take 27,648 of the SM's 65,536, which leaves room for a pass-1
+// FFT CTA of 8 (36,864) beside it (tests/test_s1_sass_budget.py).
 template <int LOGD, int QC, int PS, int MT, int NST>
-__global__ void __launch_bounds__((MT / 64 + 1) * 32, 1)
+__global__ void __maxnreg__(96)
 k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, const __grid_constant__ CUtensorMap tm) {
     using Lay = XtLay<LOGD, QC, MT>;
     constexpr int D = Lay::D, NSEG = Lay::NSEG, NR = Lay::NR, REGION = Lay::REGION, STAGE = Lay::STAGE, NW = Lay::NW;
-    constexpr int NQH = (QC >> 1) + 1;
     constexpr int NSLOT = NST;                                           // ring depth: a slot is a whole tile (NSEG * 2 boxes)
     constexpr int SLOT = STAGE;
     extern __shared__ __align__(1024) unsigned char xt_smem[];
@@ -136,8 +137,8 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
     unsigned char* const gbase = xt_smem + (sbase - (unsigned)__cvta_generic_to_shared(xt_smem));
     float2* C = reinterpret_cast<float2*>(gbase + XT_STAGES * STAGE);    // [njobs][PS]  e^{j w_v ((b - s) mod PS)}
     float2* TL = C + (size_t)p.njobs * PS;                               // [njobs][16]  e^{j w_v D j}
-    float2* PHW = TL + (size_t)p.njobs * 16;                             // [NW][njobs][4] per warp and tile: coarse phase
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(PHW + (size_t)NW * p.njobs * 4);
+    float2* PHW = TL + (size_t)p.njobs * 16;                             // [njobs][NPH] per tile: coarse phase of 16 outputs
+    unsigned long long* bars = reinterpret_cast<unsigned long long*>(PHW + (size_t)p.njobs * Lay::NPH);
     const unsigned bar0 = (unsigned)__cvta_generic_to_shared(bars);     // full[s] = bar0 + 8 s, empty[s] = bar0 + 8 (NSLOT + s)
     float2* H = reinterpret_cast<float2*>(bars + 2 * NSLOT);              // [njobs][F2H] ÷4 epilogue: carried stage-1 outputs
 
@@ -169,6 +170,7 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
         }
         if (g.f2) {
             // the stage-1 outputs in front of the first tile: only the first CTA reads them (from the stage's history)
+#pragma unroll 1
             for (int idx = tid; idx < p.njobs * Lay::F2H; idx += NW * 32) {
                 const int v = idx / Lay::F2H, i = idx - v * Lay::F2H;
                 const long long m = first - g.cj - Lay::F2H + i;
@@ -211,36 +213,36 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
     }
 
     // ---------------- consumers ----------------
-    const int jl = warp * 64 + 2 * lane;            // first of this lane's two adjacent outputs (even)
-    unsigned aoff[NQH];
+    const int jw = xt_lane_out(lane);
+    const int jl = warp * 32 + jw;                  // this lane's output within the tile
+    // window block jl + q: parity region (jl + q) & 1, row (jl + q) >> 1, its 16-byte chunks swizzled by row & 7
+    unsigned aoff[QC];
 #pragma unroll
-    for (int qh = 0; qh < NQH; qh++) {
-        const unsigned row = (unsigned)((jl >> 1) + qh);
-        aoff[qh] = row * 128u + ((row & 7u) << 4);
+    for (int q = 0; q < QC; q++) {
+        const unsigned row = (unsigned)((jl + q) >> 1);
+        aoff[q] = (unsigned)(((jl + q) & 1) * REGION) + row * 128u + ((row & 7u) << 4);
     }
     int it = 0;                                     // tiles consumed so far (the producer's sequence)
     for (long long J0 = first; J0 < own1; J0 += MT) {
-        // coarse phase table of this warp's 64 outputs: entry (job, i) = phase at output jl0 + 16 i, drift-centred
+        // coarse phases of this warp's 32 outputs: entry (job, 2 warp + i) = phase at output 32 warp + 16 i, drift-centred
         {
-            for (int e = lane; e < p.njobs * 4; e += 32) {
-                const int vv = e >> 2, i = e & 3;
+            for (int e = lane; e < p.njobs * 2; e += 32) {
+                const int vv = e >> 1, i = e & 1;
                 const XdJob& Jv = p.job[vv];
                 const int a0 = Jv.offset - (Jv.T - 1);
-                const long long im0 = (long long)a0 + (J0 + warp * 64 + i * 16 - (long long)g.cj) * D;
+                const long long im0 = (long long)a0 + (J0 + warp * 32 + i * 16 - (long long)g.cj) * D;
                 unsigned long long dr = Jv.w * (unsigned long long)PS;
                 if (p.pfb_sigma < 0) { dr -= 0x8000000000000000ULL; }
                 const long long corr = (long long)dr * (long long)(Jv.T / (2 * PS));
-                PHW[(warp * p.njobs + vv) * 4 + i] = phasor_u64(Jv.phase0 + Jv.w * (unsigned long long)im0 + (unsigned long long)corr);
+                PHW[vv * Lay::NPH + 2 * warp + i] = phasor_u64(Jv.phase0 + Jv.w * (unsigned long long)im0 + (unsigned long long)corr);
             }
         }
         const bool fast = tile_fast(J0);
 
-        // ---- accumulate: D/2 phase pairs x (QC+1) window blocks, 2 outputs x PS classes per lane, slot by slot ----
-        float2 S[2][PS];
+        // ---- accumulate: D/2 phase pairs x QC window blocks, PS classes per lane, segment by segment ----
+        float2 S[PS];
 #pragma unroll
-        for (int o = 0; o < 2; o++)
-#pragma unroll
-            for (int a = 0; a < PS; a++) { S[o][a] = make_float2(0.f, 0.f); }
+        for (int a = 0; a < PS; a++) { S[a] = make_float2(0.f, 0.f); }
         const int sl = it % NSLOT;
         const unsigned ph = (unsigned)((it / NSLOT) & 1);
         it++;
@@ -271,11 +273,11 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
             asm volatile("bar.sync 1, %0;\n" ::"n"(NW * 32) : "memory");
         }
         if (!(g.diag & 1)) {
-            xt_accumulate<LOGD, QC, PS, REGION, 0, 8, NQH>(S, g, sb, aoff);
-            xt_accumulate<LOGD, QC, PS, REGION, 8, 16, NQH>(S, g, sb + 2 * REGION, aoff);
+            xt_accumulate<LOGD, QC, PS, 0, 8>(S, g, sb, aoff);
+            xt_accumulate<LOGD, QC, PS, 8, 16>(S, g, sb + 2 * REGION, aoff);
             if constexpr (NSEG == 4) {
-                xt_accumulate<LOGD, QC, PS, REGION, 16, 24, NQH>(S, g, sb + 4 * REGION, aoff);
-                xt_accumulate<LOGD, QC, PS, REGION, 24, 32, NQH>(S, g, sb + 6 * REGION, aoff);
+                xt_accumulate<LOGD, QC, PS, 16, 24>(S, g, sb + 4 * REGION, aoff);
+                xt_accumulate<LOGD, QC, PS, 24, 32>(S, g, sb + 6 * REGION, aoff);
             }
         }
         static_assert(NSEG == 2 || NSEG == 4, "D = 32 or 64");
@@ -293,6 +295,7 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
         }
         float2* const stg = reinterpret_cast<float2*>(gbase + sl * SLOT);
         if (g.f2) {
+#pragma unroll 1
             for (int idx = tid; idx < p.njobs * Lay::F2H; idx += NW * 32) {
                 const int v = idx / Lay::F2H, i = idx - v * Lay::F2H;
                 stg[v * Lay::F2P + xt_f2_pad(i)] = H[idx];
@@ -303,44 +306,31 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
         const long long m0 = J0 + jl - (long long)g.cj;
         const int nout = p.job[0].n_out;                       // every job of a filter-bank launch has the same length
         // outputs of this CTA's run (the halo in front of it and the tail past its end belong to its neighbours)
-        const bool own0k = J0 + jl >= own0 && J0 + jl < own1, own1k = J0 + jl + 1 >= own0 && J0 + jl + 1 < own1;
-        const bool ok0 = own0k && m0 >= 0 && m0 < nout, ok1 = own1k && (m0 + 1) >= 0 && (m0 + 1) < nout;
-        const int ih = (2 * lane) >> 4, il = (2 * lane) & 15;
-        // stage-1 output y of job v at m: to the ÷4 staging, and to `out` where the next stage's history needs it
-        auto put = [&](int v, long long m, bool ok, float2 y, float2* out) {
+        const bool ok = J0 + jl >= own0 && J0 + jl < own1 && m0 >= 0 && m0 < nout;
+        const int ih = 2 * warp + (jw >> 4), il = jw & 15;
+        // stage-1 output y of job v: to the ÷4 staging, and to `out` where the next stage's history needs it
+        auto put = [&](int v, float2 y) {
             const XdJob& Jv = p.job[v];
             if (g.f2 && Jv.f2_out) {
-                // m < 0 only in the first CTA's first tile, when the first output's block is odd: the value of the history
-                stg[v * Lay::F2P + xt_f2_pad(Lay::F2H + (int)(m - m0) + jl)] = m >= 0 ? y : Jv.f2_hist[Lay::F2H + m];
-                if (ok && m >= nout - Lay::F2H) { *out = y; }
+                // m0 < 0 only in the first CTA's first tile, when the first output's block is odd: the value of the history
+                stg[v * Lay::F2P + xt_f2_pad(Lay::F2H + jl)] = m0 >= 0 ? y : Jv.f2_hist[Lay::F2H + m0];
+                if (ok && m0 >= nout - Lay::F2H) { Jv.out[m0] = y; }
             }
-            else if (ok) { *out = y; }
+            else if (ok) { Jv.out[m0] = y; }
         };
         for (int sv = 0; sv < p.nslots; sv++) {
             const int ja = p.slot_a[sv], jb = p.slot_b[sv];
-            float2 A0 = make_float2(0.f, 0.f), B0 = A0, A1 = A0, B1 = A0;
+            float2 A = make_float2(0.f, 0.f), B = A;
             const float2* cv = C + ja * PS;
 #pragma unroll
             for (int a = 0; a < PS; a++) {
                 const float2 c = cv[a];
-                A0 = ffma2(make_float2(c.x, c.x), S[0][a], A0);
-                B0 = ffma2(make_float2(c.y, c.y), S[0][a], B0);
-                A1 = ffma2(make_float2(c.x, c.x), S[1][a], A1);
-                B1 = ffma2(make_float2(c.y, c.y), S[1][a], B1);
+                A = ffma2(make_float2(c.x, c.x), S[a], A);
+                B = ffma2(make_float2(c.y, c.y), S[a], B);
             }
-            {
-                const float2 pc = PHW[(warp * p.njobs + ja) * 4 + ih];
-                const float2 p0 = cmulf(pc, TL[ja * 16 + il]), p1 = cmulf(pc, TL[ja * 16 + il + 1]);
-                float2* out = p.job[ja].out + m0;
-                put(ja, m0, ok0, cmulf(make_float2(A0.x - B0.y, A0.y + B0.x), p0), out);
-                put(ja, m0 + 1, ok1, cmulf(make_float2(A1.x - B1.y, A1.y + B1.x), p1), out + 1);
-            }
-            if (jb >= 0) {
-                const float2 pc = PHW[(warp * p.njobs + jb) * 4 + ih];
-                const float2 p0 = cmulf(pc, TL[jb * 16 + il]), p1 = cmulf(pc, TL[jb * 16 + il + 1]);
-                float2* out = p.job[jb].out + m0;
-                put(jb, m0, ok0, cmulf(make_float2(A0.x + B0.y, A0.y - B0.x), p0), out);      // conjugate coefficients
-                put(jb, m0 + 1, ok1, cmulf(make_float2(A1.x + B1.y, A1.y - B1.x), p1), out + 1);
+            put(ja, cmulf(make_float2(A.x - B.y, A.y + B.x), cmulf(PHW[ja * Lay::NPH + ih], TL[ja * 16 + il])));
+            if (jb >= 0) {                                     // conjugate coefficients
+                put(jb, cmulf(make_float2(A.x + B.y, A.y - B.x), cmulf(PHW[jb * Lay::NPH + ih], TL[jb * 16 + il])));
             }
         }
         if (g.f2) {
@@ -349,6 +339,7 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
             //      with the tap order and arithmetic of k_dfir_reg ----
             constexpr int NG = MT / 16;                        // groups of four outputs per job and tile
             const long long t0 = J0 - g.cj;                    // stage-1 index of the tile's first output (staging entry F2H)
+#pragma unroll 1
             for (int task = tid; task < p.njobs * NG; task += NW * 32) {
                 const int v = task / NG, gi = task - v * NG;
                 const XdJob& Jv = p.job[v];
@@ -378,6 +369,7 @@ k_xd_tma(const __grid_constant__ XdParams p, const __grid_constant__ XtGeom g, c
                 }
             }
             // the last F2H stage-1 outputs of the tile are the window's start in the next one
+#pragma unroll 1
             for (int idx = tid; idx < p.njobs * Lay::F2H; idx += NW * 32) {
                 const int v = idx / Lay::F2H, i = idx - v * Lay::F2H;
                 H[idx] = stg[v * Lay::F2P + xt_f2_pad(MT + i)];
