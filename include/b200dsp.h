@@ -305,7 +305,7 @@ long long b200_fe_stat(b200_fe* fe, const char* key);
  *            (same lines either way)
  *  "graph"   -1 (default) / 1: the launches behind stage 1 of a chunk are recorded; a chunk whose list was seen before
  *            replays a captured CUDA graph (decimation offsets, resampler phases and buffer parities repeat after a few
- *            chunks of any fixed size); 0 = plain launches.  "tail_split" 2 = two independent branches (halves of the VFOs)
+ *            chunks of any fixed size); 0 = plain launches.
  *  "host_direct" -1 (default): VFO outputs in b200_host_alloc buffers are stored by the kernels themselves for chunks up to
  *            4 Mi samples (no copy to enqueue), 1 always, 0 never (copy engine); IQ taps (b200_fe_bind_iq) under -1 only
  *            when their output is at most 64 KiB, since the kernel's own stores over PCIe are slower than the copy engine

@@ -878,7 +878,6 @@ extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {
     if (!strcmp(key, "graph")) { fe->sch.graph_tails = value; if (value == 0) { fe->sch.drop_graphs(); } return 0; }
     if (!strcmp(key, "graph_max_count")) { fe->sch.graph_max_count = value; return 0; }
     if (!strcmp(key, "pdl")) { kernels_set_pdl(value); fe->sch.drop_graphs(); return 0; }      // process-wide, like the kernel variants
-    if (!strcmp(key, "tail_split")) { fe->sch.tail_split = value; fe->sch.drop_graphs(); return 0; }
     if (!strcmp(key, "time_s1")) { fe->sch.time_s1 = value != 0; for (auto& t : fe->sch.timers) { t.used = 0; } return 0; }
     set_error("unknown option %s", key);
     return B200_EINVAL;

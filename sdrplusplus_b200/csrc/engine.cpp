@@ -859,9 +859,6 @@ int Scheduler::init_raw() {
 }
 Scheduler::~Scheduler() {
     drop_graphs();
-    if (tail_stream2) { cudaStreamSynchronize(tail_stream2); cudaStreamDestroy(tail_stream2); }
-    if (rec.ev_fork) { cudaEventDestroy(rec.ev_fork); }
-    if (rec.ev_join) { cudaEventDestroy(rec.ev_join); }
     for (Timer& t : timers) { for (cudaEvent_t e : t.ev) { cudaEventDestroy(e); } }
 }
 cudaEvent_t Scheduler::timer_begin(int group, cudaStream_t s) {
@@ -957,36 +954,20 @@ static int apply_pending_taps(FirCStage* f, cudaStream_t s) {
     return 0;
 }
 
-// ---- launch list of a chunk's tail section (engine.h: LaunchRec) ----
-static thread_local LaunchRec* g_rec = nullptr;      // set while Scheduler::run records instead of launching
-struct RecScope {
-    explicit RecScope(LaunchRec* r) { g_rec = r; }
-    ~RecScope() { g_rec = nullptr; }
-};
-static inline int rec_tag(const FirParams&) { return LaunchRec::T_FIR; }
-static inline int rec_tag(const PolyParams&) { return LaunchRec::T_POLY; }
-static inline int rec_tag(const FirRParams&) { return LaunchRec::T_FIRR; }
-static inline int rec_tag(const QuadParams&) { return LaunchRec::T_QUAD; }
-static inline int rec_tag(const SeqParams&) { return LaunchRec::T_SEQ; }
-static inline int rec_tag(const M2SParams&) { return LaunchRec::T_M2S; }
-static inline int rec_tag(const ScaleParams&) { return LaunchRec::T_SCALE; }
-static inline int rec_tag(const CarryParams&) { return LaunchRec::T_CARRY; }
-static inline int rec_tag(const FmIfParams&) { return LaunchRec::T_FMIF; }
-static inline int rec_tag(const RxlParams&) { return LaunchRec::T_RXL; }
-
-void LaunchRec::add(int tag, void* fn, const void* p, size_t size, int a, int b, size_t c) {
+// ---- launch list of everything behind stage 1 of a chunk (engine.h: LaunchRec) ----
+void LaunchRec::add(Launch fn, const void* p, size_t size, int a, size_t b) {
     const size_t off = (bytes.size() + 15) & ~(size_t)15;
     bytes.resize(off + size, 0);
     memcpy(bytes.data() + off, p, size);
-    items.push_back(Item{ tag, fn, off, size, a, b, c, cur_branch });
+    items.push_back(Item{ fn, off, size, a, b });
 }
 unsigned long long LaunchRec::hash() const {
-    // 64-bit multiply-xorshift over the parameter bytes and the launch arguments
+    // 64-bit multiply-xorshift over the launchers, the launch arguments and the parameter bytes
     unsigned long long h = 0x9E3779B97F4A7C15ULL ^ (unsigned long long)items.size();
     auto mix = [&](unsigned long long v) { h ^= v; h *= 0xD6E8FEB86659FD93ULL; h ^= h >> 32; };
     for (const Item& it : items) {
-        mix((unsigned long long)it.tag | ((unsigned long long)it.branch << 32)); mix((unsigned long long)(uintptr_t)it.fn); mix((unsigned long long)it.size);
-        mix((unsigned long long)(unsigned)it.a | ((unsigned long long)(unsigned)it.b << 32)); mix((unsigned long long)it.c);
+        mix((unsigned long long)(uintptr_t)it.fn); mix((unsigned long long)it.size);
+        mix((unsigned long long)(unsigned)it.a); mix((unsigned long long)it.b);
     }
     const size_t n8 = bytes.size() / 8;
     const unsigned char* b = bytes.data();
@@ -994,77 +975,77 @@ unsigned long long LaunchRec::hash() const {
     for (size_t i = n8 * 8; i < bytes.size(); i++) { mix(b[i]); }
     return h;
 }
-int LaunchRec::replay(cudaStream_t s0, long long* nlaunch) const {
-    // branch 1 (if any) forks from s0 before anything of this list runs and joins it at the end
-    bool two = false;
-    for (const Item& it : items) { two = two || it.branch != 0; }
-    if (two) {
-        if (!aux || !ev_fork || !ev_join) { set_error("launch list: no second stream"); return B200_ESTATE; }
-        B200_CK(cudaEventRecord(ev_fork, s0));
-        B200_CK(cudaStreamWaitEvent(aux, ev_fork, 0));
-    }
+int LaunchRec::replay(cudaStream_t s, long long* nlaunch) const {
     for (const Item& it : items) {
-        cudaStream_t s = it.branch ? aux : s0;
-        const void* q = bytes.data() + it.off;
-        cudaError_t e = cudaSuccess;
-        int nl = 1;
-        switch (it.tag) {
-        case T_DFR: e = launch_dfir_reg(*(const DfrParams*)q, it.a, it.b, s); break;
-        case T_FIR: e = ((cudaError_t (*)(const FirParams&, cudaStream_t))it.fn)(*(const FirParams*)q, s); break;
-        case T_POLY: e = ((cudaError_t (*)(const PolyParams&, cudaStream_t))it.fn)(*(const PolyParams*)q, s); break;
-        case T_FIRR: e = ((cudaError_t (*)(const FirRParams&, cudaStream_t))it.fn)(*(const FirRParams*)q, s); break;
-        case T_QUAD: e = launch_quad(*(const QuadParams*)q, s); break;
-        case T_SEQ: e = launch_seq(*(const SeqParams*)q, s); break;
-        case T_M2S: e = launch_m2s(*(const M2SParams*)q, s); break;
-        case T_SCALE: e = launch_scale(*(const ScaleParams*)q, s); break;
-        case T_CARRY: e = launch_carry(*(const CarryParams*)q, s); break;
-        case T_FMIF: e = launch_fmif(*(const FmIfParams*)q, s); break;
-        case T_RXL: e = launch_rxl(*(const RxlParams*)q, s); break;
-        case T_STEREO: nl = 0; e = launch_stereo(*(const StParams*)q, s, &nl); break;
-        case T_SQUELCH: nl = 0; e = launch_squelch(*(const SqParams*)q, s, &nl); break;
-        case T_FUSED: e = launch_tail_fused(*(const FtParams*)q, it.a, it.b, it.c, s); break;
-        default: set_error("launch list: unknown tag %d", it.tag); return B200_EINVAL;
-        }
+        int nl = 0;
+        cudaError_t e = it.fn(bytes.data() + it.off, it, s, &nl);
         if (e != cudaSuccess) { return cuda_fail(e, "kernel launch (tail list)"); }
         if (nlaunch) { *nlaunch += nl; }
     }
-    if (two) {
-        B200_CK(cudaEventRecord(ev_join, aux));
-        B200_CK(cudaStreamWaitEvent(s0, ev_join, 0));
-    }
     return 0;
 }
+
+// the launchers of the list: one per typed launch function
+template <class P, cudaError_t (*L)(const P&, cudaStream_t)>
+static cudaError_t launch_of(const void* p, const LaunchRec::Item&, cudaStream_t s, int* nl) {
+    *nl = 1;
+    return L(*(const P*)p, s);
+}
+template <class P, cudaError_t (*L)(const P&, cudaStream_t, int*)>        // launch_stereo, launch_squelch: more than one kernel
+static cudaError_t launch_of_n(const void* p, const LaunchRec::Item&, cudaStream_t s, int* nl) {
+    return L(*(const P*)p, s, nl);
+}
+static cudaError_t launch_of_dfr(const void* q, const LaunchRec::Item&, cudaStream_t s, int* nl) {
+    const DfrParams& p = *(const DfrParams*)q;                              // every job of a batch: the same D and T
+    *nl = 1;
+    return launch_dfir_reg(p, p.job[0].decim, p.job[0].ntaps, s);
+}
+static cudaError_t launch_of_ft(const void* q, const LaunchRec::Item& it, cudaStream_t s, int* nl) {
+    const FtParams& p = *(const FtParams*)q;
+    int max_slabs = 0;
+    for (int i = 0; i < p.njobs; i++) { max_slabs = std::max(max_slabs, p.job[i].slabs); }
+    *nl = 1;
+    return launch_tail_fused(p, max_slabs, it.a, it.b, s);                  // a, b: threads, shared memory
+}
+
+// One parameter block of the launch list: jobs go in one at a time, and the block goes into the list when it is full, when
+// the caller's key (what every job of one launch must share) changes, and at the end of a level.  `mx`: the block's largest
+// job count, if it keeps one.  Blocks start zero-filled: the list is hashed and compared as bytes.
+template <class P>
+struct Batch {
+    static const int CAP = (int)(sizeof(P::job) / sizeof(P::job[0]));
+    P p;
+    LaunchRec::Launch fn;
+    int P::*mx;
+    int a = 0;
+    size_t b = 0;                // launch arguments outside the block (LaunchRec::Item)
+    explicit Batch(LaunchRec::Launch f, int P::*m = nullptr) : fn(f), mx(m) { memset(&p, 0, sizeof(P)); }
+    void flush(LaunchRec& rec) {
+        if (p.njobs == 0) { return; }
+        rec.add(fn, &p, sizeof(P), a, b);
+        p.njobs = 0;
+        if (mx) { p.*mx = 0; }
+    }
+    // the slot of the next job; a full block, or one holding jobs under another key, goes into the list first
+    auto& next(LaunchRec& rec, bool key_changed = false) {
+        if (p.njobs > 0 && (key_changed || p.njobs == CAP)) { flush(rec); }
+        return p.job[p.njobs++];
+    }
+    // after the job is filled in: its count, and a block that is now full goes into the list (unless `eager` is false, where
+    // it waits for the next job)
+    void done(LaunchRec& rec, int n, bool eager = true) {
+        if (mx) { p.*mx = std::max(p.*mx, n); }
+        if (eager && p.njobs == CAP) { flush(rec); }
+    }
+};
+
 void Scheduler::drop_graphs() {
     for (auto& kv : graphs) { if (kv.second.exec) { cudaGraphExecDestroy(kv.second.exec); } }
     graphs.clear();
 }
 
-template <class P, class L>
-static int flush_batch(P& p, L launch, cudaStream_t s, long long& launches) {
-    if (p.njobs == 0) { return 0; }
-    if (g_rec) {
-        g_rec->add(rec_tag(p), (void*)launch, &p, sizeof(P));
-        p.njobs = 0;
-        return 0;
-    }
-    cudaError_t e = launch(p, s);
-    if (e != cudaSuccess) { return cuda_fail(e, "kernel launch"); }
-    launches++;
-    p.njobs = 0;
-    return 0;
-}
-
 int Scheduler::enable_overlap(cudaStream_t tail) {
     tail_stream = tail;
-    if (tail && !tail_stream2) {
-        int lo = 0, hi = 0, pr = 0;
-        cudaDeviceGetStreamPriorityRange(&lo, &hi);
-        if (cudaStreamGetPriority(tail, &pr) != cudaSuccess) { pr = hi; }
-        B200_CK(cudaStreamCreateWithPriority(&tail_stream2, cudaStreamNonBlocking, pr));
-        B200_CK(cudaEventCreateWithFlags(&rec.ev_fork, cudaEventDisableTiming));
-        B200_CK(cudaEventCreateWithFlags(&rec.ev_join, cudaEventDisableTiming));
-        rec.aux = tail_stream2;
-    }
     for (int i = 0; i < 2; i++) {
         if (!ev_stage1[i]) { B200_CK(cudaEventCreateWithFlags(&ev_stage1[i], cudaEventDisableTiming)); }
         if (!ev_tail[i]) { B200_CK(cudaEventCreateWithFlags(&ev_tail[i], cudaEventDisableTiming)); }
@@ -1091,9 +1072,6 @@ int Scheduler::apply_deferred(std::vector<Chain*>& chains) {
     }
     return 0;
 }
-
-template <class P>
-static inline void zero_params(P& p, bool) { memset(&p, 0, sizeof(P)); }
 
 // the recorded launch list of this chunk: first sight -> plain launches; second sight -> capture into a graph; then replay
 int Scheduler::launch_recorded(cudaStream_t ts, bool may_graph) {
@@ -1144,16 +1122,12 @@ static inline long long host_now_ns() {
     return (long long)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
-int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int count, bool carry_raw) {
-    const long long hp0 = host_now_ns();
-    // ---- wiring ----
-    const int parity = (int)(chunk_idx & 1);
-    cudaStream_t ts = tail_stream ? tail_stream : stream;
-    size_t depth = 0;
-    {
-        int rc = apply_deferred(chains);          // no-op when the caller already did it
-        if (rc) { return rc; }
-    }
+// level of a chain's first stage in the level-by-level section: an RDS branch starts at its parent's discriminator
+static size_t first_level(const Chain* c) { return c->parent ? (size_t)std::max(0, c->parent->quad_index()) : 0; }
+
+int Scheduler::wire(std::vector<Chain*>& chains, int parity) {
+    int rc = apply_deferred(chains);          // no-op when the caller already did it
+    if (rc) { return rc; }
     for (Chain* c : chains) {
         for (auto& sp : c->st) { sp->par = parity; }
     }
@@ -1162,23 +1136,92 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
         B200_CK(cudaStreamWaitEvent(stream, ev_tail[parity], 0));
     }
     trace_mark("stage1 start", stream);
-    // level of a chain's first stage in the level-by-level section: an RDS branch starts at its parent's discriminator
-    auto lvl0 = [](const Chain* c) -> size_t { return c->parent ? (size_t)std::max(0, c->parent->quad_index()) : 0; };
     for (Chain* c : chains) {
-        depth = std::max(depth, lvl0(c) + c->st.size());
         for (size_t i = 0; i < c->st.size(); i++) {
             Stage* s = c->st[i].get();
             s->out_ptr = (i + 1 < c->st.size()) ? c->st[i + 1]->in_data() : (c->out_override ? c->out_override : c->out.as<float>());
-            if (s->kind == K_XD) {
-                XdStage* x = (XdStage*)s;
-                if (x->taps_dirty) {
-                    int rc = x->upload_taps(stream);
-                    if (rc) { return rc; }
+            if (s->kind == K_XD && ((XdStage*)s)->taps_dirty && (rc = ((XdStage*)s)->upload_taps(stream))) { return rc; }
+        }
+    }
+    return 0;
+}
+
+// slots of a stage-1 batch: pair VFOs whose complex taps are exact conjugates (offsets +f / -f, same real prototype, same
+// decimation phase): they share every multiply-accumulate of stage 1 (kernels.cuh: XdParams)
+static void pair_slots(XdParams& p, XdStage* const* g, bool pair) {
+    bool used[B200_BATCH] = { false };
+    p.nslots = 0;
+    for (int v = 0; v < p.njobs; v++) {
+        if (used[v]) { continue; }
+        used[v] = true;
+        int partner = -1;
+        XdStage* a = g[v];
+        if (pair && a->w != 0) {
+            for (int u = v + 1; u < p.njobs; u++) {
+                XdStage* c = g[u];
+                if (!used[u] && c->w == (0ULL - a->w) && c->T == a->T && c->chunk_offset == a->chunk_offset &&
+                    c->n_out == a->n_out && c->h == a->h) {
+                    partner = u;
+                    used[u] = true;
+                    break;
                 }
             }
         }
+        p.slot_a[p.nslots] = (signed char)v;
+        p.slot_b[p.nslots] = (signed char)partner;
+        p.nslots++;
     }
-    // ---- stage 1: every raw-input chain, grouped by first-stage decimation so they share the IQ tile ----
+}
+
+// polyphase-filter-bank form (xd_pfb.cuh): every job on a common frequency grid fs / (2 PS), same prototype, same alignment.
+// Accept when e^{j w_v PS} is within a few 1e-6 rad (over one tap window) of the same sign.
+static void pfb_grid(XdParams& p, XdStage* const* g) {
+    XdStage* x0 = g[0];
+    for (int v = 1; v < p.njobs; v++) {
+        XdStage* xv = g[v];
+        if (xv->T != x0->T || xv->chunk_offset != x0->chunk_offset || xv->n_out != x0->n_out || xv->h != x0->h) { return; }
+    }
+    if (x0->n_out <= 0) { return; }
+    p.taps_host = x0->h.data();
+    for (int P = 1; P <= 10 && !p.pfb_ps; P++) {
+        // drift allowed per P samples so that it stays below 8e-6 rad over the T-tap window
+        const double tol_turns = (8e-6 / 6.283185307179586) * (double)P / (double)x0->T;
+        const double tol = tol_turns * 18446744073709551616.0;
+        int sg = 0;
+        bool ok = true;
+        for (int v = 0; v < p.njobs && ok; v++) {
+            const unsigned long long r = g[v]->w * (unsigned long long)P;
+            const double d0 = (double)(long long)r;                                    // distance to 0 (signed)
+            const double d1 = (double)(long long)(r - 0x8000000000000000ULL);            // distance to 1/2 turn
+            int sv = 0;
+            if (std::fabs(d0) <= tol) { sv = 1; } else if (std::fabs(d1) <= tol) { sv = -1; }
+            if (sv == 0 || (sg != 0 && sv != sg)) { ok = false; }
+            sg = sv;
+        }
+        if (!ok) { continue; }
+        // run the kernel's PS = 8 or 10 instantiation: sigma' = sigma^(PS / P)
+        for (int PS : { 8, 10 }) {
+            if (PS % P == 0) {
+                p.pfb_ps = PS;
+                p.pfb_sigma = (sg < 0 && ((PS / P) & 1)) ? -1 : 1;
+                break;
+            }
+        }
+    }
+}
+
+// The (4, 27) stage behind stage 1 is computed by k_xd_tma's ÷4 epilogue where it would otherwise run in k_dfir_reg (the
+// epilogue has its arithmetic), the stage after it is double-buffered like the one stage 1 feeds, and the chunk needs no
+// k_xd_edge patch of the stage-1 outputs.  Every other chunk -- a retune inside the tap window, another input format, a
+// launch k_xd_tma declines -- stores the stage-1 outputs and runs k_dfir_reg, reading and writing the same history.
+static FirCStage* f2_stage(const Scheduler& S, const Chain* c, const XdStage* x, int fmt) {
+    if (fmt != FMT_CF32 || S.s1_variant < 8 || S.fuse.pre_reg <= 0 || x->chunk_retuned || c->st.size() < 3) { return nullptr; }
+    if (!s1_f2_stage(c->st[1].get()) || (S.tail_stream && !c->st[2]->dbl) || (c->fp.active && c->fp.beg <= 1)) { return nullptr; }
+    return (FirCStage*)c->st[1].get();
+}
+
+// every raw-input chain, grouped by first-stage decimation so they share the IQ tile
+int Scheduler::stage1(std::vector<Chain*>& chains, const void* raw, int fmt, int count) {
     std::map<int, std::vector<XdStage*>> groups;
     std::map<XdStage*, Chain*> chain_of;
     for (Chain* c : chains) {
@@ -1188,15 +1231,6 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
             chain_of[x] = c;
         }
     }
-    // The (4, 27) stage behind stage 1 is computed by k_xd_tma's ÷4 epilogue where it would otherwise run in k_dfir_reg (the
-    // epilogue has its arithmetic), the stage after it is double-buffered like the one stage 1 feeds, and the chunk needs no
-    // k_xd_edge patch of the stage-1 outputs.  Every other chunk -- a retune inside the tap window, another input format, a
-    // launch k_xd_tma declines -- stores the stage-1 outputs and runs k_dfir_reg, reading and writing the same history.
-    auto f2_stage = [&](Chain* c, const XdStage* x) -> FirCStage* {
-        if (fmt != FMT_CF32 || s1_variant < 8 || fuse.pre_reg <= 0 || x->chunk_retuned || c->st.size() < 3) { return nullptr; }
-        if (!s1_f2_stage(c->st[1].get()) || (tail_stream && !c->st[2]->dbl) || (c->fp.active && c->fp.beg <= 1)) { return nullptr; }
-        return (FirCStage*)c->st[1].get();
-    };
     for (auto& kv : groups) {
         std::vector<XdStage*>& g = kv.second;
         for (size_t b = 0; b < g.size(); b += B200_BATCH) {
@@ -1233,7 +1267,7 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
                     p.job[v].edge_start = x->chunk_edge_start;
                 }
                 p.QP = std::max(p.QP, x->QP);
-                FirCStage* f = f2_stage(chain_of[x], x);
+                FirCStage* f = f2_stage(*this, chain_of[x], x, fmt);
                 if (f && f->n_out > 0 && (!f2_taps || *f2_taps == f->htaps)) {       // one tap set per launch
                     f2_taps = &f->htaps;
                     memcpy(p.f2_taps, f->htaps.data(), sizeof(p.f2_taps));
@@ -1246,71 +1280,9 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
                     p.job[v].f2_n = f->n_out;
                 }
             }
-            // slots: pair VFOs whose complex taps are exact conjugates (offsets +f / -f, same real prototype, same
-            // decimation phase): they share every multiply-accumulate of stage 1 (kernels.cuh: XdParams)
-            {
-                bool used[B200_BATCH] = { false };
-                p.nslots = 0;
-                for (int v = 0; v < p.njobs; v++) {
-                    if (used[v]) { continue; }
-                    used[v] = true;
-                    int partner = -1;
-                    XdStage* a = g[b + v];
-                    if (pair_conjugates && a->w != 0) {
-                        for (int u = v + 1; u < p.njobs; u++) {
-                            XdStage* c = g[b + u];
-                            if (!used[u] && c->w == (0ULL - a->w) && c->T == a->T && c->chunk_offset == a->chunk_offset &&
-                                c->n_out == a->n_out && c->h == a->h) {
-                                partner = u;
-                                used[u] = true;
-                                break;
-                            }
-                        }
-                    }
-                    p.slot_a[p.nslots] = (signed char)v;
-                    p.slot_b[p.nslots] = (signed char)partner;
-                    p.nslots++;
-                }
-            }
-            // polyphase-filter-bank form (xd_pfb.cuh): every job on a common frequency grid fs / (2 PS), same prototype,
-            // same alignment.  Accept when e^{j w_v PS} is within a few 1e-6 rad (over one tap window) of the same sign.
+            pair_slots(p, &g[b], pair_conjugates);
             p.pfb_ps = 0; p.pfb_sigma = 1; p.taps_host = nullptr;
-            if (s1_variant >= 7 && p.njobs >= 1) {
-                bool same = true;
-                XdStage* x0 = g[b];
-                for (int v = 1; v < p.njobs; v++) {
-                    XdStage* xv = g[b + v];
-                    if (xv->T != x0->T || xv->chunk_offset != x0->chunk_offset || xv->n_out != x0->n_out || xv->h != x0->h) { same = false; }
-                }
-                if (same && x0->n_out > 0) {
-                    p.taps_host = x0->h.data();
-                    for (int P = 1; P <= 10 && !p.pfb_ps; P++) {
-                        // drift allowed per P samples so that it stays below 8e-6 rad over the T-tap window
-                        const double tol_turns = (8e-6 / 6.283185307179586) * (double)P / (double)x0->T;
-                        const double tol = tol_turns * 18446744073709551616.0;
-                        int sg = 0;
-                        bool ok = true;
-                        for (int v = 0; v < p.njobs && ok; v++) {
-                            const unsigned long long r = g[b + v]->w * (unsigned long long)P;
-                            const double d0 = (double)(long long)r;                                    // distance to 0 (signed)
-                            const double d1 = (double)(long long)(r - 0x8000000000000000ULL);            // distance to 1/2 turn
-                            int sv = 0;
-                            if (std::fabs(d0) <= tol) { sv = 1; } else if (std::fabs(d1) <= tol) { sv = -1; }
-                            if (sv == 0 || (sg != 0 && sv != sg)) { ok = false; }
-                            sg = sv;
-                        }
-                        if (!ok) { continue; }
-                        // run the kernel's PS = 8 or 10 instantiation: sigma' = sigma^(PS / P)
-                        for (int PS : { 8, 10 }) {
-                            if (PS % P == 0) {
-                                p.pfb_ps = PS;
-                                p.pfb_sigma = (sg < 0 && ((PS / P) & 1)) ? -1 : 1;
-                                break;
-                            }
-                        }
-                    }
-                }
-            }
+            if (s1_variant >= 7 && p.njobs >= 1) { pfb_grid(p, &g[b]); }
             // the tiled kernel pads every job to the group's QP: all jobs of a batch must have room for it
             int variant = s1_variant;
             for (int v = 0; v < p.njobs; v++) {
@@ -1321,6 +1293,7 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
             cudaEvent_t t1 = timer_begin(0, stream);
             cudaError_t e = launch_xlate_decim(p, fmt, variant, stream, &nl, &f2);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_xlate_decim"); }
+            // ÷4-epilogue bookkeeping: which (4, 27) stages stage 1 computed this chunk
             for (int v = 0; v < p.njobs; v++) {
                 Chain* c = chain_of[g[b + v]];
                 if (c->st.size() >= 2 && c->st[1]->kind == K_FIRC) { ((FirCStage*)c->st[1].get())->s1_fused = f2 && p.job[v].f2_out; }
@@ -1333,17 +1306,288 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
             launches += nl;
         }
     }
-    // ---- raw-IQ history for the next chunk's stage 1 (same stream as stage 1) ----
-    if (carry_raw && count > 0) {
-        CarryParams rc1;
-        rc1.njobs = 1;
-        CarryJob& j = rc1.job[0];
-        j.dst = raw_hist.as<float>(); j.a = raw_hist.as<float>(); j.b = raw;
-        j.h = RAW_HIST; j.la = RAW_HIST; j.lb = count; j.esize = 2; j.bfmt = fmt; j.scale = in_scale;
-        cudaError_t e = launch_carry(rc1, stream);
-        if (e != cudaSuccess) { return cuda_fail(e, "launch_carry"); }
-        launches++;
+    return 0;
+}
+
+// raw-IQ history for the next chunk's stage 1 (same stream as stage 1)
+int Scheduler::carry_raw_hist(const void* raw, int fmt, int count) {
+    CarryParams rc1;
+    rc1.njobs = 1;
+    CarryJob& j = rc1.job[0];
+    j.dst = raw_hist.as<float>(); j.a = raw_hist.as<float>(); j.b = raw;
+    j.h = RAW_HIST; j.la = RAW_HIST; j.lb = count; j.esize = 2; j.bfmt = fmt; j.scale = in_scale;
+    cudaError_t e = launch_carry(rc1, stream);
+    if (e != cudaSuccess) { return cuda_fail(e, "launch_carry"); }
+    launches++;
+    return 0;
+}
+
+// ---- the launch list behind stage 1 ----
+// k_dfir_reg: the short decimating FIRs with the window in registers; one batch shares D, T and the taps
+static bool dfr_ok(const Stage* s, int pre_reg) {
+    if (pre_reg <= 0 || s->kind != K_FIRC || s->in_es != 2) { return false; }
+    const FirCStage* f = (const FirCStage*)s;
+    return f->decim > 1 && f->ntaps <= DFR_MAXT && dfir_reg_supported(f->decim, f->ntaps);
+}
+static void dfr_push(LaunchRec& rec, Batch<DfrParams>& dfr, const FirCStage* f) {
+    const FirJob& j0 = dfr.p.job[0];
+    FirJob& j = dfr.next(rec, j0.decim != f->decim || j0.ntaps != f->ntaps || !std::equal(f->htaps.begin(), f->htaps.end(), dfr.p.taps));
+    if (dfr.p.njobs == 1) { memcpy(dfr.p.taps, f->htaps.data(), (size_t)f->ntaps * sizeof(float)); }
+    j.in = (const float2*)f->base(); j.out = (float2*)f->out_ptr; j.taps = f->taps.as<float>();
+    j.ntaps = f->ntaps; j.decim = f->decim; j.offset = f->chunk_offset; j.n_out = f->n_out;
+    dfr.done(rec, f->n_out, false);
+}
+
+// the register FIRs in front of fused chains: one launch per level and plan stage
+static void rec_reg_firs(LaunchRec& rec, std::vector<Chain*>& chains, Batch<DfrParams>& dfr) {
+    int max_beg = 1;
+    for (Chain* c : chains) { if (c->fp.active) { max_beg = std::max(max_beg, c->fp.beg); } }
+    for (int lvl = 1; lvl < max_beg; lvl++) {
+        for (Chain* c : chains) {
+            if (!c->fp.active || lvl >= c->fp.beg) { continue; }
+            FirCStage* f = (FirCStage*)c->st[lvl].get();
+            if (f->n_out <= 0 || f->s1_fused) { continue; }
+            dfr_push(rec, dfr, f);
+        }
+        dfr.flush(rec);
     }
+}
+
+// fused tails: every FIR-like stage after stage 1 of a VFO in one launch (kernels.cuh: FtJob)
+static void rec_fused_tails(LaunchRec& rec, std::vector<Chain*>& chains, const FuseCfg& fuse, int sm_count) {
+    std::vector<Chain*> fc;
+    for (Chain* c : chains) {
+        if (c->fp.active && c->st[c->fp.beg]->n_in > 0) { fc.push_back(c); }
+    }
+    if (fc.empty()) { return; }
+    // slab size: the fewest waves the largest slabs allow, then the smallest slab that keeps that wave count
+    // (less halo-free work per CTA; the halo a slab recomputes is a fixed cost)
+    const int threads = (fuse.threads == 512 || fuse.threads == 256) ? fuse.threads : 128;
+    size_t smem = 0;
+    int ob_cap = 1 << 30;
+    for (Chain* c : fc) { smem = std::max(smem, c->fp.smem); ob_cap = std::min(ob_cap, c->fp.ob_max); }
+    // resident CTAs per SM as the device will actually place them (registers bound the 256-thread build at two)
+    static std::map<std::pair<int, size_t>, int> occ_cache;
+    int cps;
+    {
+        auto key = std::make_pair(threads, smem);
+        auto it = occ_cache.find(key);
+        if (it == occ_cache.end()) { it = occ_cache.emplace(key, tail_fused_ctas_per_sm(threads, smem)).first; }
+        cps = it->second;
+    }
+    if (cps < 1) { cps = std::max(1, std::min((int)((227 * 1024) / (smem + 1024)), 2048 / threads)); }
+    const long long slots = (long long)sm_count * cps;
+    auto total_slabs = [&](int ob) {
+        long long t = 0;
+        for (Chain* c : fc) { t += std::max(1, (c->st[c->fp.end - 1]->n_out + ob - 1) / ob); }
+        return t;
+    };
+    int ob = ob_cap;
+    if (fuse.ob_force <= 0) {
+        const long long waves = (total_slabs(ob_cap) + slots - 1) / slots;
+        int lo_ob = 4 * FT_R, hi_ob = ob_cap;           // smallest ob with total_slabs(ob) <= waves * slots
+        while (lo_ob < hi_ob) {
+            int mid = (lo_ob + hi_ob) / 2;
+            if (total_slabs(mid) <= waves * slots) { hi_ob = mid; } else { lo_ob = mid + 1; }
+        }
+        ob = hi_ob;
+    }
+    Batch<FtParams> ft(launch_of_ft);
+    ft.a = threads;
+    ft.b = smem;
+    for (Chain* c : fc) {
+        FtJob& J = ft.next(rec);
+        const int nst = c->fp.end - c->fp.beg;
+        J.nst = nst;
+        J.OB = ob;
+        J.OT0 = c->fp.ot0;
+        J.stg2 = c->fp.buf[0] + c->fp.stg2_rel; J.pad = 0;
+        J.s0_direct = c->fp.s0_direct ? 1 : 0;
+        J.stg3 = c->fp.buf[0] + 2 * c->fp.stg2_rel;
+        J.nat_off = c->fp.nat_off;
+        J.stg_floats = c->fp.stg2_rel;
+        J.taps_nat = c->fp.s0_direct ? ((FirCStage*)c->st[c->fp.beg].get())->taps.as<float>() : nullptr;
+        J.rds = nullptr; J.rds_phase0 = 0; J.rds_w = 0;
+        for (int i = 0; i < nst; i++) {
+            Stage* sg = c->st[c->fp.beg + i].get();
+            FtStage& d = J.st[i];
+            ft_describe(sg, d);
+            d.n_in = sg->n_in; d.n_out = sg->n_out;
+            d.buf = c->fp.buf[i]; d.pitch = c->fp.pitch[i]; d.tap_off = c->fp.tap_off[i]; d.qpitch = c->fp.qpitch[i];
+            if (sg->kind == K_FIRC) { d.off = ((FirCStage*)sg)->chunk_offset; }
+            if (sg->kind == K_POLY) { d.off = ((PolyStage*)sg)->chunk_offset; d.phase = ((PolyStage*)sg)->chunk_phase; }
+            if (sg->kind == K_QUAD && ((QuadStage*)sg)->side) {
+                const RxlStage* x = ((QuadStage*)sg)->side;
+                J.rds = (float2*)x->out_ptr; J.rds_phase0 = x->chunk_phase0; J.rds_w = x->w;
+            }
+            if (i > 0) {
+                d.hist_rd = sg->fh[sg->fpar].as<float>();
+                d.hist_wr = sg->fh[sg->fpar ^ 1].as<float>();
+                sg->fpar ^= 1;
+            }
+        }
+        J.src = c->st[c->fp.beg]->base();
+        J.out = c->st[c->fp.end - 1]->out_ptr;
+        J.slabs = std::max(1, (J.st[nst - 1].n_out + ob - 1) / ob);
+        ft.done(rec, 0);
+    }
+    ft.flush(rec);
+}
+
+// the remaining stages level by level: one launch per stage kind per level (batches of 16 VFOs)
+static void rec_levels(LaunchRec& rec, std::vector<Chain*>& chains, int pre_reg, Batch<DfrParams>& dfr) {
+    size_t depth = 0;
+    for (Chain* c : chains) { depth = std::max(depth, first_level(c) + c->st.size()); }
+    for (size_t lvl = 0; lvl < depth; lvl++) {
+        Batch<FirParams> fpr(launch_of<FirParams, launch_fir_reg>, &FirParams::max_out);        // decimation-1 filters with register windows
+        Batch<PolyParams> ppr(launch_of<PolyParams, launch_poly_reg>, &PolyParams::max_out);    // polyphase resamplers with register windows: one (L, M) per batch
+        Batch<FirRParams> rpr(launch_of<FirRParams, launch_firr_reg>, &FirRParams::max_out);
+        Batch<FirParams> fp(launch_of<FirParams, launch_fir_c>, &FirParams::max_out);
+        Batch<PolyParams> pp(launch_of<PolyParams, launch_poly>, &PolyParams::max_out);
+        Batch<QuadParams> qp(launch_of<QuadParams, launch_quad>, &QuadParams::max_n);
+        Batch<FirRParams> rp(launch_of<FirRParams, launch_fir_r>, &FirRParams::max_out);
+        Batch<SeqParams> sp(launch_of<SeqParams, launch_seq>);
+        Batch<M2SParams> mp(launch_of<M2SParams, launch_m2s>, &M2SParams::max_n);
+        Batch<ScaleParams> cp(launch_of<ScaleParams, launch_scale>, &ScaleParams::max_n);
+        Batch<FmIfParams> fmp(launch_of<FmIfParams, launch_fmif>, &FmIfParams::max_n);         // one bin count per batch
+        Batch<RxlParams> xlp(launch_of<RxlParams, launch_rxl>, &RxlParams::max_n);
+        Batch<StParams> stp(launch_of_n<StParams, launch_stereo>, &StParams::max_n);
+        Batch<SqParams> sqp(launch_of_n<SqParams, launch_squelch>, &SqParams::max_n);
+        for (Chain* c : chains) {
+            const size_t l0 = first_level(c);
+            if (lvl < l0 || lvl - l0 >= c->st.size()) { continue; }
+            if (c->fp.active && lvl >= 1 && (int)lvl < c->fp.end) { continue; }     // done by the fused launch
+            Stage* s = c->st[lvl - l0].get();
+            if (s->n_out <= 0) { continue; }
+            switch (s->kind) {
+            case K_XD: break;
+            case K_FIRC: {
+                FirCStage* f = (FirCStage*)s;
+                if (f->s1_fused) { break; }
+                if (dfr_ok(f, pre_reg)) { dfr_push(rec, dfr, f); break; }
+                Batch<FirParams>& b = (pre_reg > 0 && f->decim == 1 && f->in_es == 2 && f->ntaps <= 2000 && f->chunk_offset == 0) ? fpr : fp;
+                FirJob& j = b.next(rec);
+                j.in = (const float2*)f->base(); j.out = (float2*)f->out_ptr; j.taps = f->taps.as<float>();
+                j.ntaps = f->ntaps; j.decim = f->decim; j.offset = f->chunk_offset; j.n_out = f->n_out;
+                b.done(rec, f->n_out);
+                break;
+            }
+            case K_POLY: {
+                PolyStage* f = (PolyStage*)s;
+                const bool regp = pre_reg > 0 && f->in_es == 2 && f->tpp <= 512 && poly_reg_supported(f->interp, f->decim);
+                Batch<PolyParams>& b = regp ? ppr : pp;
+                PolyJob& j = b.next(rec, regp && (ppr.p.job[0].interp != f->interp || ppr.p.job[0].decim != f->decim));
+                j.in = (const float2*)f->base(); j.out = (float2*)f->out_ptr; j.bank = f->bank.as<float>();
+                j.tpp = f->tpp; j.interp = f->interp; j.decim = f->decim; j.phase0 = f->chunk_phase; j.offset0 = f->chunk_offset;
+                j.n_out = f->n_out;
+                j.bank_kl = f->bank_kl.as<float>(); j.in_len = (long long)f->hist + f->n_in;
+                b.done(rec, f->n_out);
+                break;
+            }
+            case K_QUAD: {
+                QuadStage* f = (QuadStage*)s;
+                QuadJob& j = qp.next(rec);
+                j.in = (const float2*)f->base(); j.out = f->out_ptr;
+                j.inv_dev = f->inv_dev; j.n = f->n_out;
+                j.rds = f->side ? (float2*)f->side->out_ptr : nullptr;
+                j.rds_phase0 = f->side ? f->side->chunk_phase0 : 0; j.rds_w = f->side ? f->side->w : 0;
+                qp.done(rec, f->n_out);
+                break;
+            }
+            case K_FIRR: {
+                FirRStage* f = (FirRStage*)s;
+                Batch<FirRParams>& b = (pre_reg > 0 && f->ntaps <= 2000) ? rpr : rp;
+                FirRJob& j = b.next(rec);
+                j.in = f->base(); j.out = f->out_ptr; j.taps = f->taps.as<float>();
+                j.ntaps = f->ntaps; j.n_out = f->n_out; j.stereo = f->stereo;
+                b.done(rec, f->n_out);
+                break;
+            }
+            case K_SEQ: {
+                SeqStage* f = (SeqStage*)s;
+                SeqJob& j = sp.next(rec);
+                j = f->proto;
+                j.in = (const float2*)f->in_data(); j.out = f->out_ptr; j.state = f->state.as<float>(); j.n = f->n_out;
+                sp.done(rec, f->n_out);
+                break;
+            }
+            case K_SCALE: {
+                ScaleJob& j = cp.next(rec);
+                j.in = s->in_data(); j.out = s->out_ptr; j.n = s->n_out * s->in_es; j.gain = ((ScaleStage*)s)->gain;
+                cp.done(rec, j.n);
+                break;
+            }
+            case K_STEREO: {
+                StereoStage* f = (StereoStage*)s;
+                StJob& j = stp.next(rec);
+                j.in = f->base(); j.out = (float2*)f->out_ptr; j.taps = f->taps.as<float2>(); j.p = f->p.as<float2>(); j.vco = f->vco.as<float2>();
+                j.state = f->state.as<float>(); j.ntaps = f->ntaps; j.delay = f->delay; j.n = f->n_out;
+                j.alpha = f->alpha; j.beta = f->beta; j.min_freq = f->min_freq; j.max_freq = f->max_freq;
+                stp.done(rec, f->n_out);
+                break;
+            }
+            case K_RXL: {
+                RxlStage* f = (RxlStage*)s;
+                if (c->parent && lvl == l0) { break; }      // an RDS branch's: its parent's discriminator stored it
+                RxlJob& j = xlp.next(rec);
+                j.in = f->in_data(); j.out = (float2*)f->out_ptr; j.n = f->n_out; j.phase0 = f->chunk_phase0; j.w = f->w;
+                xlp.done(rec, f->n_out);
+                break;
+            }
+            case K_FMIF: {
+                FmIfStage* f = (FmIfStage*)s;
+                FmIfJob& j = fmp.next(rec, fmp.p.job[0].bins != f->bins);
+                j.in = (const float2*)f->base(); j.out = (float2*)f->out_ptr; j.win = f->win.as<float>(); j.tw = f->tw.as<float2>();
+                j.n = f->n_out; j.bins = f->bins;
+                fmp.done(rec, f->n_out);
+                break;
+            }
+            case K_SQUELCH: {
+                SquelchStage* f = (SquelchStage*)s;
+                SqJob& j = sqp.next(rec);
+                j.in = (const float2*)f->in_data(); j.out = (float2*)f->out_ptr; j.partial = f->partial.as<float>(); j.n = f->n_out; j.level = f->level;
+                sqp.done(rec, f->n_out);
+                break;
+            }
+            case K_M2S: {
+                M2SJob& j = mp.next(rec);
+                j.in = s->in_data(); j.out = s->out_ptr; j.n = s->n_out;
+                mp.done(rec, s->n_out);
+                break;
+            }
+            }
+        }
+        // the order of these launches is part of the plan: programmatic dependent launch overlaps each with the one before
+        dfr.flush(rec); fpr.flush(rec); ppr.flush(rec); rpr.flush(rec); fp.flush(rec); pp.flush(rec); qp.flush(rec);
+        rp.flush(rec); sp.flush(rec); mp.flush(rec); cp.flush(rec); fmp.flush(rec); xlp.flush(rec); stp.flush(rec); sqp.flush(rec);
+    }
+}
+
+// history carry (the memmove at the end of every reference process())
+static void rec_history_carry(LaunchRec& rec, std::vector<Chain*>& chains) {
+    Batch<CarryParams> cp(launch_of<CarryParams, launch_carry>);
+    for (Chain* c : chains) {
+        for (auto& sp : c->st) {
+            Stage* s = sp.get();
+            if (s->kind == K_XD || s->hist <= 0 || s->fmid) { continue; }
+            if (s->n_in <= 0 && !s->dbl) { continue; }      // a double-buffered stage always hands its history over
+            CarryJob& j = cp.next(rec);
+            memset(&j, 0, sizeof(j));
+            j.dst = s->other_base(); j.a = s->base(); j.b = s->in_data();
+            j.h = s->hist; j.la = s->hist; j.lb = s->n_in; j.esize = s->in_es; j.bfmt = -1; j.scale = 0.0f;
+            cp.done(rec, 0);
+        }
+    }
+    cp.flush(rec);
+}
+
+int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int count, bool carry_raw) {
+    const long long hp0 = host_now_ns();
+    const int parity = (int)(chunk_idx & 1);
+    cudaStream_t ts = out_stream();
+    int rc;
+    if ((rc = wire(chains, parity)) || (rc = stage1(chains, raw, fmt, count))) { return rc; }
+    if (carry_raw && count > 0 && (rc = carry_raw_hist(raw, fmt, count))) { return rc; }
     if (tail_stream) {
         B200_CK(cudaEventRecord(ev_stage1[parity], stream));
         B200_CK(cudaStreamWaitEvent(ts, ev_stage1[parity], 0));
@@ -1352,435 +1596,15 @@ int Scheduler::run(std::vector<Chain*>& chains, const void* raw, int fmt, int co
     const long long hp1 = host_now_ns();
     host_ns[0] += hp1 - hp0;
     cudaEvent_t t_tail = timer_begin(1, ts);
-    // The launches of this section are recorded, then replayed: as a captured CUDA graph when the same list was seen before
-    // (one cudaGraphLaunch instead of seven to ten launches), and in `tail_split` independent branches -- the chains of the
-    // first and of the second half of the VFOs on two streams -- because every kernel here is latency-bound at a fraction
-    // of the machine: two half-size chains side by side finish well before one full-size chain.
-    const int nsplit = (tail_split > 1 && tail_stream && tail_stream2 && chains.size() >= 4) ? 2 : 1;
-    const bool use_rec = nsplit > 1 || graph_tails > 0 || (graph_tails < 0 && count <= graph_max_count);
-    if (use_rec) { rec.clear(); }
-    RecScope rec_scope(use_rec ? &rec : nullptr);
-    std::vector<Chain*>& all_chains = chains;
-    auto tail_section = [&](std::vector<Chain*>& chains) -> int {
-    // ---- short decimating FIRs with the window in registers (k_dfir_reg): one launch per level and plan stage ----
-    DfrParams dfr;
-    memset(&dfr, 0, sizeof(dfr));
-    int dfr_D = 0, dfr_T = 0;
-    const std::vector<float>* dfr_taps = nullptr;
-    auto dfr_flush = [&]() -> int {
-        if (dfr.njobs == 0) { return 0; }
-        if (g_rec) { g_rec->add(LaunchRec::T_DFR, nullptr, &dfr, sizeof(dfr), dfr_D, dfr_T); }
-        else {
-            cudaError_t e = launch_dfir_reg(dfr, dfr_D, dfr_T, ts);
-            if (e != cudaSuccess) { return cuda_fail(e, "launch_dfir_reg"); }
-            launches++;
-        }
-        dfr.njobs = 0; dfr.max_out = 0;
-        return 0;
-    };
-    auto dfr_push = [&](FirCStage* f) -> int {
-        if (dfr.njobs > 0 && (dfr_D != f->decim || dfr_T != f->ntaps || *dfr_taps != f->htaps || dfr.njobs == B200_BATCH)) {
-            int rc = dfr_flush();
-            if (rc) { return rc; }
-        }
-        if (dfr.njobs == 0) {
-            dfr_D = f->decim; dfr_T = f->ntaps; dfr_taps = &f->htaps;
-            memcpy(dfr.taps, f->htaps.data(), (size_t)f->ntaps * sizeof(float));
-        }
-        FirJob& j = dfr.job[dfr.njobs++];
-        j.in = (const float2*)f->base(); j.out = (float2*)f->out_ptr; j.taps = f->taps.as<float>();
-        j.ntaps = f->ntaps; j.decim = f->decim; j.offset = f->chunk_offset; j.n_out = f->n_out;
-        dfr.max_out = std::max(dfr.max_out, f->n_out);
-        return 0;
-    };
-    auto dfr_ok = [&](const Stage* s) {
-        if (fuse.pre_reg <= 0 || s->kind != K_FIRC || s->in_es != 2) { return false; }
-        const FirCStage* f = (const FirCStage*)s;
-        return f->decim > 1 && f->ntaps <= DFR_MAXT && dfir_reg_supported(f->decim, f->ntaps);
-    };
-    {
-        int max_beg = 1;
-        for (Chain* c : chains) { if (c->fp.active) { max_beg = std::max(max_beg, c->fp.beg); } }
-        for (int lvl = 1; lvl < max_beg; lvl++) {
-            for (Chain* c : chains) {
-                if (!c->fp.active || lvl >= c->fp.beg) { continue; }
-                FirCStage* f = (FirCStage*)c->st[lvl].get();
-                if (f->n_out <= 0 || f->s1_fused) { continue; }
-                int rc = dfr_push(f);
-                if (rc) { return rc; }
-            }
-            int rc = dfr_flush();
-            if (rc) { return rc; }
-        }
-    }
-    // ---- fused tails: every FIR-like stage after stage 1 of a VFO in one launch (kernels.cuh: FtJob) ----
-    {
-        std::vector<Chain*> fc;
-        for (Chain* c : chains) {
-            if (c->fp.active && c->st[c->fp.beg]->n_in > 0) { fc.push_back(c); }
-        }
-        if (!fc.empty()) {
-            // slab size: the fewest waves the largest slabs allow, then the smallest slab that keeps that wave count
-            // (less halo-free work per CTA; the halo a slab recomputes is a fixed cost)
-            const int threads = (fuse.threads == 512 || fuse.threads == 256) ? fuse.threads : 128;
-            size_t smem = 0;
-            int ob_cap = 1 << 30;
-            for (Chain* c : fc) { smem = std::max(smem, c->fp.smem); ob_cap = std::min(ob_cap, c->fp.ob_max); }
-            // resident CTAs per SM as the device will actually place them (registers bound the 256-thread build at two)
-            static std::map<std::pair<int, size_t>, int> occ_cache;
-            int cps;
-            {
-                auto key = std::make_pair(threads, smem);
-                auto it = occ_cache.find(key);
-                if (it == occ_cache.end()) { it = occ_cache.emplace(key, tail_fused_ctas_per_sm(threads, smem)).first; }
-                cps = it->second;
-            }
-            if (cps < 1) { cps = std::max(1, std::min((int)((227 * 1024) / (smem + 1024)), 2048 / threads)); }
-            const long long slots = (long long)sm_count * cps;
-            auto total_slabs = [&](int ob) {
-                long long t = 0;
-                for (Chain* c : fc) { t += std::max(1, (c->st[c->fp.end - 1]->n_out + ob - 1) / ob); }
-                return t;
-            };
-            int ob = ob_cap;
-            if (fuse.ob_force <= 0) {
-                const long long waves = (total_slabs(ob_cap) + slots - 1) / slots;
-                int lo_ob = 4 * FT_R, hi_ob = ob_cap;           // smallest ob with total_slabs(ob) <= waves * slots
-                while (lo_ob < hi_ob) {
-                    int mid = (lo_ob + hi_ob) / 2;
-                    if (total_slabs(mid) <= waves * slots) { hi_ob = mid; } else { lo_ob = mid + 1; }
-                }
-                ob = hi_ob;
-            }
-            FtParams fpar;
-            memset(&fpar, 0, sizeof(fpar));
-            fpar.dbg = nullptr;
-            static long long* g_ft_dbg = nullptr;
-            static int g_ft_dbg_on = -1;
-            if (g_ft_dbg_on < 0) { const char* e = getenv("B200_FT_CLOCKS"); g_ft_dbg_on = (e && *e == '1') ? 1 : 0; }
-            if (g_ft_dbg_on) {
-                if (!g_ft_dbg) { cudaMalloc(&g_ft_dbg, 32 * sizeof(long long)); cudaMemset(g_ft_dbg, 0, 32 * sizeof(long long)); }
-                else {
-                    long long h[32];
-                    cudaMemcpy(h, g_ft_dbg, sizeof(h), cudaMemcpyDeviceToHost);      // previous launch (synchronising: debug only)
-                    fprintf(stderr, "[b200 ft clocks]");
-                    for (int i = 1; i < 10 && h[i]; i++) { fprintf(stderr, " s%d %lld", i - 1, h[i] - h[i - 1]); }
-                    fprintf(stderr, " | sub-tiles (wait, compute, sync):");
-                    for (int k = 0; k < 4 && h[16 + 3 * k]; k++) {
-                        fprintf(stderr, " [%lld %lld %lld]", h[16 + 3 * k] - (k ? h[15 + 3 * k] : h[0]), h[17 + 3 * k] - h[16 + 3 * k], h[18 + 3 * k] - h[17 + 3 * k]);
-                    }
-                    fprintf(stderr, "\n");
-                }
-                fpar.dbg = g_ft_dbg;
-            }
-            int max_slabs = 0;
-            auto flush = [&]() -> int {
-                if (fpar.njobs == 0) { return 0; }
-                if (g_rec) { g_rec->add(LaunchRec::T_FUSED, nullptr, &fpar, sizeof(fpar), max_slabs, threads, smem); }
-                else {
-                    cudaError_t e = launch_tail_fused(fpar, max_slabs, threads, smem, ts);
-                    if (e != cudaSuccess) { return cuda_fail(e, "launch_tail_fused"); }
-                    launches++;
-                }
-                fpar.njobs = 0;
-                max_slabs = 0;
-                return 0;
-            };
-            for (Chain* c : fc) {
-                FtJob& J = fpar.job[fpar.njobs++];
-                const int nst = c->fp.end - c->fp.beg;
-                J.nst = nst;
-                J.OB = ob;
-                J.OT0 = c->fp.ot0;
-                J.stg2 = c->fp.buf[0] + c->fp.stg2_rel; J.pad = 0;
-                J.s0_direct = c->fp.s0_direct ? 1 : 0;
-                J.stg3 = c->fp.buf[0] + 2 * c->fp.stg2_rel;
-                J.nat_off = c->fp.nat_off;
-                J.stg_floats = c->fp.stg2_rel;
-                J.taps_nat = c->fp.s0_direct ? ((FirCStage*)c->st[c->fp.beg].get())->taps.as<float>() : nullptr;
-                J.rds = nullptr; J.rds_phase0 = 0; J.rds_w = 0;
-                for (int i = 0; i < nst; i++) {
-                    Stage* sg = c->st[c->fp.beg + i].get();
-                    FtStage& d = J.st[i];
-                    ft_describe(sg, d);
-                    d.n_in = sg->n_in; d.n_out = sg->n_out;
-                    d.buf = c->fp.buf[i]; d.pitch = c->fp.pitch[i]; d.tap_off = c->fp.tap_off[i]; d.qpitch = c->fp.qpitch[i];
-                    if (sg->kind == K_FIRC) { d.off = ((FirCStage*)sg)->chunk_offset; }
-                    if (sg->kind == K_POLY) { d.off = ((PolyStage*)sg)->chunk_offset; d.phase = ((PolyStage*)sg)->chunk_phase; }
-                    if (sg->kind == K_QUAD && ((QuadStage*)sg)->side) {
-                        const RxlStage* x = ((QuadStage*)sg)->side;
-                        J.rds = (float2*)x->out_ptr; J.rds_phase0 = x->chunk_phase0; J.rds_w = x->w;
-                    }
-                    if (i > 0) {
-                        d.hist_rd = sg->fh[sg->fpar].as<float>();
-                        d.hist_wr = sg->fh[sg->fpar ^ 1].as<float>();
-                        sg->fpar ^= 1;
-                    }
-                }
-                J.src = c->st[c->fp.beg]->base();
-                J.out = c->st[c->fp.end - 1]->out_ptr;
-                J.slabs = std::max(1, (J.st[nst - 1].n_out + ob - 1) / ob);
-                max_slabs = std::max(max_slabs, J.slabs);
-                if (fpar.njobs == B200_BATCH) { int rc = flush(); if (rc) { return rc; } }
-            }
-            int rc = flush();
-            if (rc) { return rc; }
-        }
-    }
-    // ---- remaining stages level by level: one launch per stage kind per level (batches of 16 VFOs) ----
-    for (size_t lvl = 0; lvl < depth; lvl++) {
-        // zero-filled: the parameter blocks are hashed as a whole when the launch list is recorded
-        FirParams fp; zero_params(fp, use_rec);
-        FirParams fpr; zero_params(fpr, use_rec);                   // decimation-1 filters with register windows
-        PolyParams pp; zero_params(pp, use_rec);
-        PolyParams ppr; zero_params(ppr, use_rec);                  // polyphase resamplers with register windows: one (L, M) per batch
-        FirRParams rpr; zero_params(rpr, use_rec);
-        QuadParams qp; zero_params(qp, use_rec);
-        FirRParams rp; zero_params(rp, use_rec);
-        SeqParams sp; zero_params(sp, use_rec);
-        M2SParams mp; zero_params(mp, use_rec);
-        ScaleParams cp2; zero_params(cp2, use_rec);
-        StParams stp; zero_params(stp, use_rec);
-        SqParams sqp; zero_params(sqp, use_rec);
-        FmIfParams fmp; zero_params(fmp, use_rec);                  // one bin count per batch
-        RxlParams xlp; zero_params(xlp, use_rec);
-        auto sq_flush = [&]() -> int {
-            if (sqp.njobs == 0) { return 0; }
-            int nl = 0;
-            if (g_rec) { g_rec->add(LaunchRec::T_SQUELCH, nullptr, &sqp, sizeof(sqp)); }
-            else {
-                cudaError_t e = launch_squelch(sqp, ts, &nl);
-                if (e != cudaSuccess) { return cuda_fail(e, "launch_squelch"); }
-            }
-            launches += nl;
-            sqp.njobs = 0; sqp.max_n = 0;
-            return 0;
-        };
-        auto st_flush = [&]() -> int {
-            if (stp.njobs == 0) { return 0; }
-            int nl = 0;
-            if (g_rec) { g_rec->add(LaunchRec::T_STEREO, nullptr, &stp, sizeof(stp)); }
-            else {
-                cudaError_t e = launch_stereo(stp, ts, &nl);
-                if (e != cudaSuccess) { return cuda_fail(e, "launch_stereo"); }
-            }
-            launches += nl;
-            stp.njobs = 0; stp.max_n = 0;
-            return 0;
-        };
-        for (Chain* c : chains) {
-            const size_t l0 = lvl0(c);
-            if (lvl < l0 || lvl - l0 >= c->st.size()) { continue; }
-            if (c->fp.active && lvl >= 1 && (int)lvl < c->fp.end) { continue; }     // done by the fused launch
-            Stage* s = c->st[lvl - l0].get();
-            int rc = 0;
-            switch (s->kind) {
-            case K_XD: break;
-            case K_FIRC: {
-                FirCStage* f = (FirCStage*)s;
-                if (f->n_out <= 0 || f->s1_fused) { break; }
-                if (dfr_ok(f)) { rc = dfr_push(f); break; }
-                if (fuse.pre_reg > 0 && f->decim == 1 && f->in_es == 2 && f->ntaps <= 2000 && f->chunk_offset == 0) {
-                    FirJob& jr = fpr.job[fpr.njobs++];
-                    jr.in = (const float2*)f->base(); jr.out = (float2*)f->out_ptr; jr.taps = f->taps.as<float>();
-                    jr.ntaps = f->ntaps; jr.decim = 1; jr.offset = 0; jr.n_out = f->n_out;
-                    fpr.max_out = std::max(fpr.max_out, f->n_out);
-                    if (fpr.njobs == B200_BATCH) { rc = flush_batch(fpr, launch_fir_reg, ts, launches); fpr.max_out = 0; }
-                    break;
-                }
-                FirJob& j = fp.job[fp.njobs++];
-                j.in = (const float2*)f->base(); j.out = (float2*)f->out_ptr; j.taps = f->taps.as<float>();
-                j.ntaps = f->ntaps; j.decim = f->decim; j.offset = f->chunk_offset; j.n_out = f->n_out;
-                fp.max_out = std::max(fp.max_out, f->n_out);
-                if (fp.njobs == B200_BATCH) { rc = flush_batch(fp, launch_fir_c, ts, launches); fp.max_out = 0; }
-                break;
-            }
-            case K_POLY: {
-                PolyStage* f = (PolyStage*)s;
-                if (f->n_out <= 0) { break; }
-                const bool regp = fuse.pre_reg > 0 && f->in_es == 2 && f->tpp <= 512 && poly_reg_supported(f->interp, f->decim);
-                if (regp && ppr.njobs > 0 && (ppr.job[0].interp != f->interp || ppr.job[0].decim != f->decim)) {
-                    rc = flush_batch(ppr, launch_poly_reg, ts, launches); ppr.max_out = 0;
-                    if (rc) { break; }
-                }
-                PolyJob& j = regp ? ppr.job[ppr.njobs++] : pp.job[pp.njobs++];
-                j.in = (const float2*)f->base(); j.out = (float2*)f->out_ptr; j.bank = f->bank.as<float>();
-                j.tpp = f->tpp; j.interp = f->interp; j.decim = f->decim; j.phase0 = f->chunk_phase; j.offset0 = f->chunk_offset;
-                j.n_out = f->n_out;
-                j.bank_kl = f->bank_kl.as<float>(); j.in_len = (long long)f->hist + f->n_in;
-                if (regp) {
-                    ppr.max_out = std::max(ppr.max_out, f->n_out);
-                    if (ppr.njobs == B200_BATCH) { rc = flush_batch(ppr, launch_poly_reg, ts, launches); ppr.max_out = 0; }
-                    break;
-                }
-                pp.max_out = std::max(pp.max_out, f->n_out);
-                if (pp.njobs == B200_BATCH) { rc = flush_batch(pp, launch_poly, ts, launches); pp.max_out = 0; }
-                break;
-            }
-            case K_QUAD: {
-                QuadStage* f = (QuadStage*)s;
-                if (f->n_out <= 0) { break; }
-                QuadJob& j = qp.job[qp.njobs++];
-                j.in = (const float2*)f->base(); j.out = f->out_ptr;
-                j.inv_dev = f->inv_dev; j.n = f->n_out;
-                j.rds = f->side ? (float2*)f->side->out_ptr : nullptr;
-                j.rds_phase0 = f->side ? f->side->chunk_phase0 : 0; j.rds_w = f->side ? f->side->w : 0;
-                qp.max_n = std::max(qp.max_n, f->n_out);
-                if (qp.njobs == B200_BATCH) { rc = flush_batch(qp, launch_quad, ts, launches); qp.max_n = 0; }
-                break;
-            }
-            case K_FIRR: {
-                FirRStage* f = (FirRStage*)s;
-                if (f->n_out <= 0) { break; }
-                if (fuse.pre_reg > 0 && f->ntaps <= 2000) {
-                    FirRJob& jr = rpr.job[rpr.njobs++];
-                    jr.in = f->base(); jr.out = f->out_ptr; jr.taps = f->taps.as<float>();
-                    jr.ntaps = f->ntaps; jr.n_out = f->n_out; jr.stereo = f->stereo;
-                    rpr.max_out = std::max(rpr.max_out, f->n_out);
-                    if (rpr.njobs == B200_BATCH) { rc = flush_batch(rpr, launch_firr_reg, ts, launches); rpr.max_out = 0; }
-                    break;
-                }
-                FirRJob& j = rp.job[rp.njobs++];
-                j.in = f->base(); j.out = f->out_ptr; j.taps = f->taps.as<float>();
-                j.ntaps = f->ntaps; j.n_out = f->n_out; j.stereo = f->stereo;
-                rp.max_out = std::max(rp.max_out, f->n_out);
-                if (rp.njobs == B200_BATCH) { rc = flush_batch(rp, launch_fir_r, ts, launches); rp.max_out = 0; }
-                break;
-            }
-            case K_SEQ: {
-                SeqStage* f = (SeqStage*)s;
-                if (f->n_out <= 0) { break; }
-                SeqJob& j = sp.job[sp.njobs++];
-                j = f->proto;
-                j.in = (const float2*)f->in_data(); j.out = f->out_ptr; j.state = f->state.as<float>(); j.n = f->n_out;
-                if (sp.njobs == B200_BATCH) { rc = flush_batch(sp, launch_seq, ts, launches); }
-                break;
-            }
-            case K_SCALE: {
-                if (s->n_out <= 0) { break; }
-                ScaleJob& j = cp2.job[cp2.njobs++];
-                j.in = s->in_data(); j.out = s->out_ptr; j.n = s->n_out * s->in_es; j.gain = ((ScaleStage*)s)->gain;
-                cp2.max_n = std::max(cp2.max_n, j.n);
-                if (cp2.njobs == B200_BATCH) { rc = flush_batch(cp2, launch_scale, ts, launches); cp2.max_n = 0; }
-                break;
-            }
-            case K_STEREO: {
-                StereoStage* f = (StereoStage*)s;
-                if (f->n_out <= 0) { break; }
-                StJob& j = stp.job[stp.njobs++];
-                j.in = f->base(); j.out = (float2*)f->out_ptr; j.taps = f->taps.as<float2>(); j.p = f->p.as<float2>(); j.vco = f->vco.as<float2>();
-                j.state = f->state.as<float>(); j.ntaps = f->ntaps; j.delay = f->delay; j.n = f->n_out;
-                j.alpha = f->alpha; j.beta = f->beta; j.min_freq = f->min_freq; j.max_freq = f->max_freq;
-                stp.max_n = std::max(stp.max_n, f->n_out);
-                if (stp.njobs == B200_BATCH) { rc = st_flush(); }
-                break;
-            }
-            case K_RXL: {
-                RxlStage* f = (RxlStage*)s;
-                if (f->n_out <= 0 || (c->parent && lvl == l0)) { break; }      // an RDS branch's: its parent's discriminator stored it
-                RxlJob& j = xlp.job[xlp.njobs++];
-                j.in = f->in_data(); j.out = (float2*)f->out_ptr; j.n = f->n_out; j.phase0 = f->chunk_phase0; j.w = f->w;
-                xlp.max_n = std::max(xlp.max_n, f->n_out);
-                if (xlp.njobs == B200_BATCH) { rc = flush_batch(xlp, launch_rxl, ts, launches); xlp.max_n = 0; }
-                break;
-            }
-            case K_FMIF: {
-                FmIfStage* f = (FmIfStage*)s;
-                if (f->n_out <= 0) { break; }
-                if (fmp.njobs > 0 && fmp.job[0].bins != f->bins) {
-                    rc = flush_batch(fmp, launch_fmif, ts, launches); fmp.max_n = 0;
-                    if (rc) { break; }
-                }
-                FmIfJob& j = fmp.job[fmp.njobs++];
-                j.in = (const float2*)f->base(); j.out = (float2*)f->out_ptr; j.win = f->win.as<float>(); j.tw = f->tw.as<float2>();
-                j.n = f->n_out; j.bins = f->bins;
-                fmp.max_n = std::max(fmp.max_n, f->n_out);
-                if (fmp.njobs == B200_BATCH) { rc = flush_batch(fmp, launch_fmif, ts, launches); fmp.max_n = 0; }
-                break;
-            }
-            case K_SQUELCH: {
-                SquelchStage* f = (SquelchStage*)s;
-                if (f->n_out <= 0) { break; }
-                SqJob& j = sqp.job[sqp.njobs++];
-                j.in = (const float2*)f->in_data(); j.out = (float2*)f->out_ptr; j.partial = f->partial.as<float>(); j.n = f->n_out; j.level = f->level;
-                sqp.max_n = std::max(sqp.max_n, f->n_out);
-                if (sqp.njobs == B200_BATCH) { rc = sq_flush(); }
-                break;
-            }
-            case K_M2S: {
-                if (s->n_out <= 0) { break; }
-                M2SJob& j = mp.job[mp.njobs++];
-                j.in = s->in_data(); j.out = s->out_ptr; j.n = s->n_out;
-                mp.max_n = std::max(mp.max_n, s->n_out);
-                if (mp.njobs == B200_BATCH) { rc = flush_batch(mp, launch_m2s, ts, launches); mp.max_n = 0; }
-                break;
-            }
-            }
-            if (rc) { return rc; }
-        }
-        int rc;
-        if ((rc = dfr_flush())) { return rc; }
-        if ((rc = flush_batch(fpr, launch_fir_reg, ts, launches))) { return rc; }
-        if ((rc = flush_batch(ppr, launch_poly_reg, ts, launches))) { return rc; }
-        if ((rc = flush_batch(rpr, launch_firr_reg, ts, launches))) { return rc; }
-        if ((rc = flush_batch(fp, launch_fir_c, ts, launches))) { return rc; }
-        if ((rc = flush_batch(pp, launch_poly, ts, launches))) { return rc; }
-        if ((rc = flush_batch(qp, launch_quad, ts, launches))) { return rc; }
-        if ((rc = flush_batch(rp, launch_fir_r, ts, launches))) { return rc; }
-        if ((rc = flush_batch(sp, launch_seq, ts, launches))) { return rc; }
-        if ((rc = flush_batch(mp, launch_m2s, ts, launches))) { return rc; }
-        if ((rc = flush_batch(cp2, launch_scale, ts, launches))) { return rc; }
-        if ((rc = flush_batch(fmp, launch_fmif, ts, launches))) { return rc; }
-        if ((rc = flush_batch(xlp, launch_rxl, ts, launches))) { return rc; }
-        if ((rc = st_flush())) { return rc; }
-        if ((rc = sq_flush())) { return rc; }
-    }
-    // ---- history carry (the memmove at the end of every reference process()) ----
-    CarryParams cp;
-    zero_params(cp, use_rec);
-    auto push = [&](const CarryJob& j) -> int {
-        cp.job[cp.njobs++] = j;
-        if (cp.njobs == CARRY_BATCH) { return flush_batch(cp, launch_carry, ts, launches); }
-        return 0;
-    };
-    for (Chain* c : chains) {
-        for (auto& sp : c->st) {
-            Stage* s = sp.get();
-            if (s->kind == K_XD || s->hist <= 0 || s->fmid) { continue; }
-            if (s->n_in <= 0 && !s->dbl) { continue; }      // a double-buffered stage always hands its history over
-            CarryJob j;
-            memset(&j, 0, sizeof(j));
-            j.dst = s->other_base(); j.a = s->base(); j.b = s->in_data();
-            j.h = s->hist; j.la = s->hist; j.lb = s->n_in; j.esize = s->in_es; j.bfmt = -1; j.scale = 0.0f;
-            int rc = push(j);
-            if (rc) { return rc; }
-        }
-    }
-    int rcf = flush_batch(cp, launch_carry, ts, launches);
-    if (rcf) { return rcf; }
-    return 0;
-    };    // tail_section
-    if (nsplit == 1) {
-        rec.cur_branch = 0;
-        int rcs = tail_section(all_chains);
-        if (rcs) { return rcs; }
-    }
-    else {
-        size_t half = (all_chains.size() + 1) / 2;
-        while (half < all_chains.size() && all_chains[half]->parent) { half++; }     // an RDS branch stays with its parent
-        std::vector<Chain*> ga(all_chains.begin(), all_chains.begin() + half), gb(all_chains.begin() + half, all_chains.end());
-        rec.cur_branch = 0;
-        int rcs = tail_section(ga);
-        if (rcs) { return rcs; }
-        rec.cur_branch = 1;
-        if ((rcs = tail_section(gb))) { return rcs; }
-        rec.cur_branch = 0;
-    }
-    if (use_rec) {
-        g_rec = nullptr;
-        int rcg = launch_recorded(ts, graph_tails > 0 || (graph_tails < 0 && count <= graph_max_count));
-        if (rcg) { return rcg; }
-    }
+    // Everything behind stage 1 goes into one launch list, then replays: as a captured CUDA graph when the same list was
+    // seen before (one cudaGraphLaunch instead of seven to ten launches), else as plain launches.
+    rec.clear();
+    Batch<DfrParams> dfr(launch_of_dfr, &DfrParams::max_out);     // k_dfir_reg, in front of fused chains and in the levels
+    rec_reg_firs(rec, chains, dfr);
+    rec_fused_tails(rec, chains, fuse, sm_count);
+    rec_levels(rec, chains, fuse.pre_reg, dfr);
+    rec_history_carry(rec, chains);
+    if ((rc = launch_recorded(ts, graph_tails > 0 || (graph_tails < 0 && count <= graph_max_count)))) { return rc; }
     if (t_tail) { B200_CK(cudaEventRecord(t_tail, ts)); }
     trace_mark("tails+carry done", ts);
     if (tail_stream) { B200_CK(cudaEventRecord(ev_tail[parity], ts)); }

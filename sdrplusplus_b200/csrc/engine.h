@@ -296,15 +296,14 @@ void clear_stage_state(Stage& s);
 // seven to ten kernel launches).  Decimation offsets / resampler phases / buffer parities make the list periodic over a few
 // chunks for any fixed chunk size, so a handful of graphs covers a stream.
 struct LaunchRec {
-    enum Tag { T_DFR = 1, T_FIR, T_POLY, T_FIRR, T_QUAD, T_SEQ, T_M2S, T_SCALE, T_STEREO, T_SQUELCH, T_FUSED, T_CARRY, T_FMIF, T_RXL };
-    struct Item { int tag; void* fn; size_t off, size; int a, b; size_t c; int branch; };
-    int cur_branch = 0;              // items added now belong to this branch (0: the stream of the list, 1: `aux`, forked and joined)
-    cudaStream_t aux = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    struct Item;
+    // a typed launch function behind a type-erased pointer (engine.cpp: launch_of); *nl = the kernels it enqueued
+    typedef cudaError_t (*Launch)(const void* params, const Item& it, cudaStream_t s, int* nl);
+    struct Item { Launch fn; size_t off, size; int a; size_t b; };    // a, b: launch arguments outside the parameter block
     std::vector<Item> items;
     std::vector<unsigned char> bytes;
     void clear() { items.clear(); bytes.clear(); }
-    void add(int tag, void* fn, const void* p, size_t size, int a = 0, int b = 0, size_t c = 0);
+    void add(Launch fn, const void* p, size_t size, int a = 0, size_t b = 0);
     unsigned long long hash() const;
     int replay(cudaStream_t s, long long* nlaunch) const;     // the real launches, in order
 };
@@ -322,11 +321,9 @@ struct Scheduler {
     int enable_overlap(cudaStream_t tail);
     long long launches = 0;
     long long s1_f2_jobs = 0;    // VFO-chunks whose (4, 27) stage stage 1 computed (k_xd_tma's ÷4 epilogue; b200_fe_stat "s1_f2_jobs")
-    // launch-list replay (LaunchRec): -1 = for chunks up to graph_max_count samples, 0 = never, 1 = always
+    // CUDA graphs of the launch list (LaunchRec): -1 = for chunks up to graph_max_count samples, 0 = never (plain replay), 1 = always
     int graph_tails = -1;
     int graph_max_count = 1 << 30;
-    int tail_split = 1;          // 2: the chains of the two halves of the VFOs run as independent branches on two streams (measured: the chain gets 20 % shorter, the step does not -- the other streams slow down by as much)
-    cudaStream_t tail_stream2 = nullptr;
     struct GraphEntry { cudaGraphExec_t exec = nullptr; long long launches = 0; std::vector<unsigned char> key; };
     std::unordered_map<unsigned long long, GraphEntry> graphs;
     LaunchRec rec;
@@ -358,6 +355,10 @@ struct Scheduler {
     // raw: device pointer to the chunk (format fmt) for chains with raw_input(); typed chains were fed by
     // copying into st[0]->in_data() beforehand.  counts were planned already (Chain::plan).
     int run(std::vector<Chain*>& chains, const void* raw, int fmt, int count, bool carry_raw);
+    // the steps of run() in front of the launch list: output pointers and tap uploads, stage 1, the raw-IQ history carry
+    int wire(std::vector<Chain*>& chains, int parity);
+    int stage1(std::vector<Chain*>& chains, const void* raw, int fmt, int count);
+    int carry_raw_hist(const void* raw, int fmt, int count);
     int apply_deferred(std::vector<Chain*>& chains);   // pending FIR taps; call before Chain::plan()
     int reset_raw();
 };

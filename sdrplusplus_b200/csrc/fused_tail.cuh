@@ -295,8 +295,6 @@ __global__ void __launch_bounds__(NT, 2) k_tail_fused(const __grid_constant__ Ft
         for (int k = tid; k < (S.ntap_f >> 2); k += NT) { tp[k] = __ldg(src + k); }
     }
     __syncthreads();
-    const bool dbg = p.dbg && blockIdx.x == 1 && blockIdx.y == 0 && tid == 0;
-    if (dbg) { p.dbg[0] = clock64(); }
 
     for (int s = 0; s < nst; s++) {
         const FtStage& S = J.st[s];
@@ -344,15 +342,11 @@ __global__ void __launch_bounds__(NT, 2) k_tail_fused(const __grid_constant__ Ft
                     const int t0 = mlo + k * tl, t1 = min(mhi, t0 + tl);
                     if (tid == 0 && k + 2 < nsub) { issue_bulk(k + 2); }
                     ft_mbar_wait(&s_bar[k % 3], (unsigned)((k / 3) & 1));
-                    if (dbg && k < 4) { p.dbg[16 + 3 * k] = clock64(); }
                     ft_phase_direct<NT>(S, dst, sm + J.nat_off, reinterpret_cast<const float2*>(ring(k)), g_first(k) & 1, t0, t1);
-                    if (dbg && k < 4) { p.dbg[17 + 3 * k] = clock64(); }
                     __syncthreads();
-                    if (dbg && k < 4) { p.dbg[18 + 3 * k] = clock64(); }
                 }
             }
             __syncthreads();
-            if (dbg) { p.dbg[1 + s] = clock64(); }
             if (!fin && last) {
                 const FtStage& N = J.st[s + 1];
                 const int i0 = N.n_in - N.hist;
@@ -491,7 +485,6 @@ __global__ void __launch_bounds__(NT, 2) k_tail_fused(const __grid_constant__ Ft
             if (s == 0) { __syncthreads(); }
         }
         __syncthreads();
-        if (dbg) { p.dbg[1 + s] = clock64(); }
         // ---- the last slab hands the next stage's final `hist` inputs to the next chunk ----
         if (!fin && last) {
             const FtStage& N = J.st[s + 1];

@@ -172,7 +172,7 @@ struct FtJob {
     unsigned long long rds_phase0, rds_w;
     FtStage st[FT_MAXST];
 };
-struct FtParams { int njobs; int pad; long long* dbg; FtJob job[B200_BATCH]; };   // dbg: optional per-stage clock64() of CTA (1,0)
+struct FtParams { int njobs; int pad; FtJob job[B200_BATCH]; };
 
 #if defined(__CUDACC__)
 #define FT_HD __host__ __device__

@@ -1,18 +1,18 @@
 #!/bin/bash
 # occupancy experiment: device-resident value of the bench workload with fewer persistent stage-1 CTAs (SMs left free for the
-# kernels of the other streams), tail split on / off
+# kernels of the other streams)
 cd "$(dirname "$0")/.."
-mkdir -p gpurun_out
-for cfg in "0:1" "132:1" "120:1" "104:1" "120:2" "104:2" "88:2"; do
-    IFS=: read ctas sp <<< "$cfg"
-    timeout 300 python bench.py --quick --steps 8 --warmup 4 --no-cpu --c3 0 --c4 0 --ft tail_split=$sp,s1_ctas=$ctas > gpurun_out/prio_tmp.json 2> gpurun_out/prio_tmp.err
-    python - "$ctas" "$sp" <<'PY'
+out=$(mktemp -d)
+trap 'rm -rf "$out"' EXIT
+for ctas in 0 132 120 104 88; do
+    timeout 300 python bench.py --quick --steps 8 --warmup 4 --no-cpu --c3 0 --c4 0 --ft s1_ctas=$ctas > "$out/prio.json" 2> "$out/prio.err"
+    python - "$ctas" "$out/prio.json" <<'PY'
 import json,sys
 try:
-    d=json.loads(open('gpurun_out/prio_tmp.json').read().strip().splitlines()[-1])
+    d=json.loads(open(sys.argv[2]).read().strip().splitlines()[-1])
     g={x['group']:round(x['avg_ms']*1e3,1) for x in d['roofline']['by_group']}
-    print(sys.argv[1:], round(d['value']), g)
+    print(sys.argv[1], round(d['value']), g)
 except Exception as e:
-    print(sys.argv[1:], 'failed', e)
+    print(sys.argv[1], 'failed', e)
 PY
 done
