@@ -298,8 +298,8 @@ long long b200_fe_stat(b200_fe* fe, const char* key);
  *            the fused launch k_tail_fused, tuned by "ft_threads", "ft_obmax", "ft_ob", "ft_smem_kb", "ft_direct");
  *            1 = one tiled kernel per stage, 0 = one thread per output.  Before VFOs are added.
  *  "overlap" 1 = tails of chunk k overlap stage 1 of chunk k+1 on a second stream (default).  Before VFOs are added.
- *  "fft"     1 = register-resident four-step passes (default), 0 = shared-memory radix-8 passes; "fft_async" 1 = own stream;
- *            "fft_cta" 8 (default) or 4 transforms per CTA; "fft_serial" 1 = stage 1 of a chunk waits for its spectrum branch;
+ *  "fft"     1 = register-resident four-step passes (default), 0 = shared-memory radix-8 passes; "fft_cta" 8 (default)
+ *            or 4 transforms per CTA;
  *            "fft_v" 1 (default) = a frame begun in earlier chunks is staged by copies and joins its chunk's batch, twiddles
  *            from shared memory; 0 = the frame is converted to cf32 and transformed alone, twiddles from global memory
  *            (same lines either way)

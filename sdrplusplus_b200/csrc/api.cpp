@@ -281,18 +281,13 @@ struct b200_fe {
     cudaStream_t own_stream = nullptr, copy_stream = nullptr, fft_stream = nullptr, tail_stream = nullptr, join_stream = nullptr;
     cudaEvent_t ev_tail_done[FE_SLOTS] = {};
     cudaEvent_t ev_fft_go = nullptr, ev_fft_done = nullptr, ev_lines_free = nullptr;
-    bool overlap = true;         // tails of chunk k on their own stream, overlapping stage 1 of chunk k+1
     bool lines_busy = false;
-    float* lines_override = nullptr;   // this chunk: dB lines go straight to the caller's device buffer
-    bool fft_async = true;       // spectrum branch on its own stream, concurrent with the VFO branch
-    bool fft_join_pending = false;
     std::vector<std::unique_ptr<VfoSlot>> vfos;
     std::mutex mtx;
     DevBuf in_dev[FE_SLOTS];
     // FFT branch
     bool fft_on = false;
     FftCore fft;
-    double fft_rate = 0;
     int skip = 0;
     DevBuf frame, lines;
     int max_lines = 0;
@@ -310,7 +305,6 @@ struct b200_fe {
     bool slot_used[FE_SLOTS] = {};
     int max_inflight = 2;                    // chunks between submit and wait (option "inflight", up to FE_SLOTS)
     unsigned long long nsub = 0, nwait = 0;
-    int fft_serial = 0;                      // 1: stage 1 of a chunk starts when the spectrum branch of that chunk is done
     int host_direct = -1;                    // pinned host outputs written by the kernels themselves: -1 small chunks, 0 never, 1 always
     long long host_ns[4] = { 0, 0, 0, 0 };   // host time of submit(): [0] checks + plans, [1] spectrum branch, [2] Scheduler::run, [3] join + outputs
     float scale16 = 1.0f / 32768.0f, scale8 = 1.0f / 128.0f;
@@ -337,22 +331,6 @@ struct b200_fe {
     DevBuf tap_stage[FE_SLOTS];              // outputs that leave through a copy: one region per tap, 16-byte aligned
 };
 
-// (float)x * scale for the integer input formats: 1/32768 and 1/128 unless the caller set the scale of a
-// compressed-stream packet (b200_fe_set_ingest_scale)
-static float fe_ingest_scale(const b200_fe* fe, int fmt) {
-    if (fmt == B200_FMT_CS16) { return fe->scale16; }
-    if (fmt == B200_FMT_CS8) { return fe->scale8; }
-    return 0.0f;
-}
-
-static int fe_alloc_fft(b200_fe* fe) {
-    int rc;
-    if ((rc = fe->frame.alloc((size_t)fe->fft.nz * sizeof(float2)))) { return rc; }
-    long long interval = (long long)fe->fft.nz + fe->skip;
-    fe->max_lines = (int)(fe->max_eff / interval) + 2;
-    return fe->lines.alloc((size_t)fe->max_lines * fe->fft.size * sizeof(float));
-}
-
 extern "C" b200_fe* b200_fe_create(double samplerate, int max_chunk) {
     if (ensure_device()) { return nullptr; }
     if (samplerate <= 0 || max_chunk < 1) { set_error("bad samplerate/max_chunk"); return nullptr; }
@@ -369,8 +347,6 @@ extern "C" b200_fe* b200_fe_create(double samplerate, int max_chunk) {
     cudaDeviceGetStreamPriorityRange(&lo, &hi);                     // lo: numerically largest = least urgent
     int pt = 2, pm = 1, pf = 0;
     if (const char* e = getenv("B200_STREAM_PRIO")) { sscanf(e, "%d,%d,%d", &pt, &pm, &pf); }
-    if (const char* e = getenv("B200_FFT_SERIAL")) { fe->fft_serial = atoi(e); }
-    if (const char* e = getenv("B200_FFT_CTA")) { kernels_set_fft_cta(atoi(e)); }
     auto prio = [&](int level) { int p = lo - level; return p < hi ? hi : p; };
     bool ok = cudaStreamCreateWithPriority(&fe->own_stream, cudaStreamNonBlocking, prio(pm)) == cudaSuccess &&
               cudaStreamCreateWithFlags(&fe->copy_stream, cudaStreamNonBlocking) == cudaSuccess &&
@@ -417,10 +393,6 @@ extern "C" void b200_fe_destroy(b200_fe* fe) {
     if (fe->ev_lines_free) { cudaEventDestroy(fe->ev_lines_free); }
     if (fe->tail_stream) { cudaStreamDestroy(fe->tail_stream); }
     if (fe->join_stream) { cudaStreamDestroy(fe->join_stream); }
-    for (int i = 0; i < 2; i++) {
-        if (fe->sch.ev_stage1[i]) { cudaEventDestroy(fe->sch.ev_stage1[i]); }
-        if (fe->sch.ev_tail[i]) { cudaEventDestroy(fe->sch.ev_tail[i]); }
-    }
     if (fe->ev_fft_go) { cudaEventDestroy(fe->ev_fft_go); }
     if (fe->ev_fft_done) { cudaEventDestroy(fe->ev_fft_done); }
     if (fe->own_stream) { cudaStreamDestroy(fe->own_stream); }
@@ -483,11 +455,12 @@ extern "C" int b200_fe_set_fft(b200_fe* fe, int size, double rate, int window) {
     if (rate <= 0) { set_error("bad fft rate"); return B200_EINVAL; }
     int nz, skip;
     fft_frame_params(fe->fs_eff, size, rate, nz, skip);
-    int rc = fe->fft.create(size, nz, window, (int)(fe->max_eff / ((long long)nz + skip)) + 2);
+    const int max_lines = (int)(fe->max_eff / ((long long)nz + skip)) + 2;
+    int rc = fe->fft.create(size, nz, window, max_lines);
     if (rc) { return rc; }
     fe->skip = skip;
-    fe->fft_rate = rate;
-    if ((rc = fe_alloc_fft(fe))) { return rc; }
+    fe->max_lines = max_lines;
+    if ((rc = fe->frame.alloc((size_t)nz * sizeof(float2))) || (rc = fe->lines.alloc((size_t)max_lines * size * sizeof(float)))) { return rc; }
     // Reshaper restart (iq_frontend.cpp:269-279): framing restarts at the current stream position
     fe->fstart = fe->pos;
     fe->fft_on = true;
@@ -565,8 +538,10 @@ static int build_vfo_chain(b200_fe* fe, VfoSlot* v) {
     return 0;
 }
 
-// what one chunk of `count` samples can put into a VFO's output buffer, in 8-byte elements
+// what one chunk of `count` samples can put into the output buffer of a VFO, an RDS output (8-byte elements) or an IQ tap
+// (one sample per sample of the effective stream)
 static int vfo_out_bound(const b200_fe* fe, const VfoSlot* v, int count) {
+    if (is_tap(v)) { return std::max(count, 0); }
     if (is_rds_out(v)) {
         // the parent's stages up to its discriminator (the IF blocks are 1:1), then the branch
         const Chain& p = fe->vfos[v->rds_parent]->chain;
@@ -582,6 +557,17 @@ static int vfo_out_bound(const b200_fe* fe, const VfoSlot* v, int count) {
     return v->rds ? b200_rds_demod_max_out(n) : n;
 }
 
+// the first unused id of the one id space of VFOs, IQ taps and RDS outputs (an unused slot is always a fresh VfoSlot: removing
+// or unbinding an id replaces its slot), else a new one at the end; -1 when all B200_MAX_VFOS are taken
+static int new_slot_id(b200_fe* fe) {
+    for (size_t i = 0; i < fe->vfos.size(); i++) {
+        if (!fe->vfos[i]->used) { return (int)i; }
+    }
+    if (fe->vfos.size() >= B200_MAX_VFOS) { return -1; }
+    fe->vfos.push_back(std::make_unique<VfoSlot>());
+    return (int)fe->vfos.size() - 1;
+}
+
 extern "C" int b200_fe_add_vfo(b200_fe* fe, const b200_vfo_cfg* cfg) {
     if (!fe || !cfg) { set_error("null argument"); return B200_EINVAL; }
     if (cfg->out_samplerate <= 0 || cfg->bandwidth <= 0) { set_error("bad VFO rates"); return B200_EINVAL; }
@@ -589,16 +575,8 @@ extern "C" int b200_fe_add_vfo(b200_fe* fe, const b200_vfo_cfg* cfg) {
         set_error("bad AM agc_mode"); return B200_EINVAL;
     }
     std::lock_guard<std::mutex> lck(fe->mtx);
-    int id = -1;
-    for (size_t i = 0; i < fe->vfos.size(); i++) {
-        if (!fe->vfos[i]->used) { id = (int)i; break; }
-    }
-    if (id < 0) {
-        if (fe->vfos.size() >= B200_MAX_VFOS) { set_error("too many VFOs"); return B200_ECAP; }
-        fe->vfos.push_back(std::make_unique<VfoSlot>());
-        id = (int)fe->vfos.size() - 1;
-    }
-    else { fe->vfos[id] = std::make_unique<VfoSlot>(); }
+    const int id = new_slot_id(fe);
+    if (id < 0) { set_error("too many VFOs"); return B200_ECAP; }
     VfoSlot* v = fe->vfos[id].get();
     v->cfg = *cfg;
     int rc = build_vfo_chain(fe, v);
@@ -617,14 +595,6 @@ static VfoSlot* get_vfo(b200_fe* fe, int id) {
     if (v && is_tap(v)) { set_error("id %d is an IQ tap, not a VFO", id); return nullptr; }
     if (v && is_rds_out(v)) { set_error("id %d is the RDS output of VFO %d, not a VFO", id, v->rds_parent); return nullptr; }
     return v;
-}
-static int new_slot_id(b200_fe* fe) {
-    for (size_t i = 0; i < fe->vfos.size(); i++) {
-        if (!fe->vfos[i]->used) { return (int)i; }
-    }
-    if (fe->vfos.size() >= B200_MAX_VFOS) { return -1; }
-    fe->vfos.push_back(std::make_unique<VfoSlot>());
-    return (int)fe->vfos.size() - 1;
 }
 
 // BroadcastFM::setRDSOut calls reset() (broadcast_fm.h:121-142): the discriminator's previous sample, the stereo stage (pilot
@@ -707,16 +677,8 @@ extern "C" int b200_fe_bind_iq(b200_fe* fe, int sample_type, float scalar) {
             return cuda_fail(cudaGetLastError(), "IQ tap stream/event creation");
         }
     }
-    int id = -1;
-    for (size_t i = 0; i < fe->vfos.size(); i++) {
-        if (!fe->vfos[i]->used) { id = (int)i; break; }
-    }
-    if (id < 0) {
-        if (fe->vfos.size() >= B200_MAX_VFOS) { set_error("too many VFOs and IQ taps"); return B200_ECAP; }
-        fe->vfos.push_back(std::make_unique<VfoSlot>());
-        id = (int)fe->vfos.size() - 1;
-    }
-    else { fe->vfos[id] = std::make_unique<VfoSlot>(); }
+    const int id = new_slot_id(fe);
+    if (id < 0) { set_error("too many VFOs and IQ taps"); return B200_ECAP; }
     VfoSlot* v = fe->vfos[id].get();
     v->tap_type = sample_type;
     v->tap_scalar = (sample_type == B200_IQ_CF32 || sample_type == B200_IQ_U8) ? 0.0f : scalar;
@@ -799,9 +761,7 @@ extern "C" int b200_fe_vfo_count(b200_fe* fe) {
 }
 extern "C" int b200_fe_vfo_max_out(b200_fe* fe, int id, int count) {
     VfoSlot* v = get_slot(fe, id);
-    if (!v) { return B200_EINVAL; }
-    if (is_tap(v)) { return std::max(count, 0); }      // one sample per sample of the effective stream
-    return vfo_out_bound(fe, v, count);
+    return v ? vfo_out_bound(fe, v, count) : B200_EINVAL;
 }
 extern "C" int b200_fe_fft_max_lines(b200_fe* fe, int count) {
     if (!fe || !fe->fft_on) { return 0; }
@@ -842,7 +802,6 @@ extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {
         return 0;
     }
     if (!strcmp(key, "pair")) { fe->sch.pair_conjugates = value != 0; return 0; }
-    if (!strcmp(key, "fft_async")) { fe->fft_async = value != 0; return 0; }
     if (!strcmp(key, "s1_mt")) { kernels_set_xd_tile(value); return 0; }
     if (!strcmp(key, "s1_cps")) { kernels_set_xd_cps(value); return 0; }
     if (!strcmp(key, "s1_stages")) { kernels_set_xd_tma_stages(value); return 0; }
@@ -868,7 +827,6 @@ extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {
         fe->max_inflight = value;
         return 0;
     }
-    if (!strcmp(key, "fft_serial")) { fe->fft_serial = value; return 0; }
     if (!strcmp(key, "fft_v")) {
         if (value != 0 && value != 1) { set_error("fft_v: 0 or 1"); return B200_EINVAL; }
         std::lock_guard<std::mutex> lck(fe->mtx);
@@ -1091,57 +1049,247 @@ static int apply_pending(b200_fe* fe) {
     return 0;
 }
 
-static int fe_fft_chunk(b200_fe* fe, const void* dptr, int fmt, int count, int* nlines) {
-    *nlines = 0;
-    if (!fe->fft_on) { fe->pos += (unsigned long long)count; return 0; }
-    const unsigned long long pos = fe->pos, end = pos + (unsigned long long)count;
+// One chunk on its way through b200_fe_submit: what its steps hand each other
+struct FeChunk {
+    int slot = 0;                            // input slot and event set: nsub % FE_SLOTS
+    b200_outputs* out = nullptr;
+    // the chunk as submitted (in: on the device once fe_upload has run), and the effective stream behind the pre-processing
+    // that the spectrum branch, the IQ taps and the VFOs read.  scale: (float)x * scale for the integer formats
+    const void* in = nullptr, *ein = nullptr;
+    int fmt = 0, count = 0, efmt = 0, ecount = 0;
+    float scale = 0.0f, escale = 0.0f;
+    std::vector<Chain*> chains;              // every VFO's chain, a bound RDS branch right behind its parent's
+    std::vector<int> ids;                    // the VFO id of chains[k]
+    std::vector<int> taps;                   // IQ tap ids
+    bool direct = false;                     // device outputs
+    bool kernel_out[B200_MAX_VFOS] = {};     // by id: the output's last kernel writes the caller's buffer, no copy
+    std::vector<size_t> tap_off;             // taps[k]'s region in tap_stage[slot] when it leaves by a copy
+    bool fft_forked = false, tap_forked = false;
+    int nlines = 0;                          // FFT lines the chunk completes
+};
+
+// the used slots: VFO chains, each bound RDS branch right behind the VFO whose discriminator feeds it (Chain::parent); IQ taps
+static void fe_branches(b200_fe* fe, FeChunk& c) {
+    for (size_t i = 0; i < fe->vfos.size(); i++) {
+        const VfoSlot* v = fe->vfos[i].get();
+        if (!v->used || is_rds_out(v)) { continue; }
+        if (is_tap(v)) { c.taps.push_back((int)i); continue; }
+        c.chains.push_back(&fe->vfos[i]->chain); c.ids.push_back((int)i);
+        if (v->rds_child >= 0) { c.chains.push_back(&fe->vfos[v->rds_child]->chain); c.ids.push_back(v->rds_child); }
+    }
+}
+
+// the spectrum frames that complete by stream position `end`: the frame at fstart and those behind it, nz + skip apart
+static int fft_frames_by(const b200_fe* fe, unsigned long long end) {
     const unsigned long long nz = (unsigned long long)fe->fft.nz, interval = nz + (unsigned long long)fe->skip;
-    const int bps = bytes_per_sample(fmt);
-    const float isc = fe_ingest_scale(fe, fmt);
-    fe->fft.plan.in_scale = isc;
-    cudaStream_t main_s = fe->sch.stream;
-    // with overlapped tails the spectrum branch must be on its own stream (its output leaves through the tail stream)
-    const bool async = fe->fft_async || fe->sch.tail_stream != nullptr;
-    float* const lines_base = fe->lines_override ? fe->lines_override : fe->lines.as<float>();
-    cudaStream_t s = async ? fe->fft_stream : main_s;
-    bool forked = false;
+    return fe->fstart + nz <= end ? (int)((end - fe->fstart - nz) / interval) + 1 : 0;
+}
+
+// every capacity check against the exact counts, before anything is enqueued and before any state moves
+static int fe_check_outputs(b200_fe* fe, FeChunk& c) {
+    const b200_outputs* out = c.out;
+    // samples that reach the FFT branch and the VFOs: the chunk itself, or what the input decimator makes of it
+    c.ecount = (fe->decim > 1) ? fe->pre.peek(c.count) : c.count;
+    if (c.ecount < 0) { set_error("input decimator is not a FIR cascade"); return B200_ESTATE; }
+    for (const std::vector<int>* ids : { &c.ids, &c.taps }) {
+        for (int id : *ids) {
+            const VfoSlot* v = fe->vfos[id].get();
+            const int bound = vfo_out_bound(fe, v, c.ecount);
+            if (out->vfo_out[id] == nullptr || out->vfo_cap[id] < bound) {
+                set_error("%s %d output buffer too small: need room for %d samples (b200_fe_vfo_max_out)", is_tap(v) ? "IQ tap" : "VFO", id, bound);
+                return B200_ECAP;
+            }
+        }
+    }
+    if (fe->fft_on) {
+        const int need = fft_frames_by(fe, fe->pos + (unsigned long long)c.ecount);
+        if (need > fe->max_lines) { set_error("FFT line buffer overflow: %d lines complete in this chunk, room for %d", need, fe->max_lines); return B200_ECAP; }
+        if (need > 0 && (out->fft_out == nullptr || out->fft_cap_lines < need)) {
+            set_error("FFT output buffer too small: %d lines complete in this chunk", need);
+            return B200_ECAP;
+        }
+    }
+    return 0;
+}
+
+// a host chunk goes to in_dev[slot] on the copy stream, once the chunk that used the slot before is done with it; the main
+// stream waits for the copy
+static int fe_upload(b200_fe* fe, FeChunk& c, const void* iq, int in_mem) {
+    c.in = iq;
+    if (in_mem != B200_MEM_HOST || c.count == 0) { return 0; }
+    const size_t in_bytes = (size_t)c.count * bytes_per_sample(c.fmt);
+    DevBuf& buf = fe->in_dev[c.slot];
+    if (buf.bytes < in_bytes) {
+        B200_CK(cudaStreamSynchronize(fe->sch.stream));
+        int rc = buf.alloc(std::max(in_bytes, (size_t)fe->max_chunk * bytes_per_sample(c.fmt)), false);
+        if (rc) { return rc; }
+    }
+    if (fe->slot_used[c.slot]) { B200_CK(cudaStreamWaitEvent(fe->copy_stream, fe->ev_compute[c.slot], 0)); }
+    trace_mark("h2d start", fe->copy_stream);
+    B200_CK(cudaMemcpyAsync(buf.p, iq, in_bytes, cudaMemcpyHostToDevice, fe->copy_stream));
+    trace_mark("h2d done", fe->copy_stream);
+    B200_CK(cudaEventRecord(fe->ev_h2d[c.slot], fe->copy_stream));
+    B200_CK(cudaStreamWaitEvent(fe->sch.stream, fe->ev_h2d[c.slot], 0));
+    c.in = buf.p;
+    return 0;
+}
+
+// The chains' deferred filter changes, then IQFrontEnd's pre-processing chain (iq_frontend.cpp:32-39): decimator -> DC
+// blocker -> conjugate, on the main stream.  Then every chain plans the chunk.
+static int fe_preprocess(b200_fe* fe, FeChunk& c) {
+    int rc = fe->sch.apply_deferred(c.chains);
+    if (rc) { return rc; }
+    cudaStream_t s = fe->sch.stream;
+    c.ein = c.in; c.efmt = c.fmt; c.escale = c.scale;
+    const bool any = fe->decim > 1 || fe->dc_block || fe->invert_iq;
+    if (any && fe->slot_used[c.slot]) { B200_CK(cudaStreamWaitEvent(s, fe->ev_compute[c.slot], 0)); }     // pp[slot] of two chunks ago
+    if (fe->decim > 1) {
+        // the decimator's output is one buffer: the last chunk's IQ taps may still be reading it
+        if (fe->tap_read_pre) { B200_CK(cudaStreamWaitEvent(s, fe->ev_tap_done, 0)); }
+        cudaError_t e = launch_convert_cf32(c.in, c.fmt, (float2*)fe->pre.st[0]->in_data(), c.count, c.scale, s);
+        if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
+        fe->sch.launches++;
+        fe->pre.plan(c.count);
+        std::vector<Chain*> pc{ &fe->pre };
+        const long long l0 = fe->sch_pre.launches;
+        fe->sch_pre.stream = s;
+        if ((rc = fe->sch_pre.run(pc, nullptr, FMT_CF32, c.count, false))) { return rc; }
+        fe->sch.launches += fe->sch_pre.launches - l0;
+        c.ein = fe->pre.out.p; c.efmt = FMT_CF32; c.escale = 0.0f;
+    }
+    if (fe->dc_block || fe->invert_iq) {
+        const size_t need = ((size_t)fe->max_eff + 8) * sizeof(float2);
+        if (fe->pp[c.slot].bytes < need && (rc = fe->pp[c.slot].alloc(need, false))) { return rc; }
+        const int nseg_max = fe->max_eff / 4096 + 2;
+        if (!fe->dc_state.p && ((rc = fe->dc_state.alloc(16)) || (rc = fe->dc_segA.alloc((size_t)nseg_max * sizeof(float), false)) ||
+                                (rc = fe->dc_segB.alloc((size_t)nseg_max * sizeof(float2), false)))) { return rc; }
+        DcbParams dp;
+        memset(&dp, 0, sizeof(dp));
+        dp.in = c.ein; dp.out = fe->pp[c.slot].as<float2>(); dp.fmt = c.efmt; dp.count = c.ecount; dp.in_scale = c.escale;
+        dp.rate = (float)(50.0 / fe->fs_eff);                      // genDCBlockRate (iq_frontend.h:55-57)
+        dp.dc_on = fe->dc_block ? 1 : 0; dp.conj_on = fe->invert_iq ? 1 : 0;
+        dp.state = fe->dc_state.as<float2>(); dp.segA = fe->dc_segA.as<float>(); dp.segB = fe->dc_segB.as<float2>();
+        dp.nseg = (c.ecount + 4095) / 4096;
+        int nl = 0;
+        cudaError_t e = launch_preproc(dp, s, &nl);
+        if (e != cudaSuccess) { return cuda_fail(e, "launch_preproc"); }
+        fe->sch.launches += nl;
+        c.ein = fe->pp[c.slot].p; c.efmt = FMT_CF32; c.escale = 0.0f;
+    }
+    for (Chain* ch : c.chains) { ch->plan(ch->parent ? ch->parent->st[ch->parent->quad_index()]->n_out : c.ecount); }
+    return 0;
+}
+
+// Whether the last kernel of output `id` writes the caller's buffer itself, with no copy on the join stream: always for
+// device outputs; a host buffer from b200_host_alloc (stored over PCIe) under "host_direct" 1, or under -1 for chunks up to
+// 4 Mi samples whose output is at most max_bytes -- large ones keep the copy engine: a kernel's own stores moved a 1 Mi-sample
+// CF32 IQ tap (8 MiB) at a third of its rate.
+static bool kernel_writes_out(const b200_fe* fe, const FeChunk& c, int id, size_t elem_bytes, size_t max_bytes) {
+    if (c.direct) { return true; }
+    if (fe->host_direct == 0 || (fe->host_direct < 0 && (c.ecount > (1 << 22) || (size_t)c.ecount * elem_bytes > max_bytes))) { return false; }
+    return host_buffer_is_ours(c.out->vfo_out[id], (size_t)c.out->vfo_cap[id] * elem_bytes);
+}
+
+static void fe_route_outputs(b200_fe* fe, FeChunk& c) {
+    for (size_t k = 0; k < c.chains.size(); k++) {
+        const int id = c.ids[k];
+        c.kernel_out[id] = kernel_writes_out(fe, c, id, (size_t)c.chains[k]->out_es * sizeof(float), SIZE_MAX);
+        // an RDS VFO's chain output stays in the chain: RDSDemod reads it there and writes the caller's buffer itself
+        c.chains[k]->out_override = (c.kernel_out[id] && !fe->vfos[id]->rds) ? (float*)c.out->vfo_out[id] : nullptr;
+    }
+    for (int id : c.taps) { c.kernel_out[id] = kernel_writes_out(fe, c, id, iq_tap_bytes(fe->vfos[id]->tap_type), 64 << 10); }
+}
+
+// IQ taps: k_iq_tap reads the effective stream once and stores every tap, on its own stream so that neither the VFO branch
+// nor the spectrum branch waits for it.  A tap whose kernel does not write the caller's buffer fills its region of
+// tap_stage[slot], copied out on the join stream.  tap_stage[slot] was last read by the copies of chunk nsub - FE_SLOTS,
+// which b200_fe_wait has seen complete.
+static int fe_iq_taps(b200_fe* fe, FeChunk& c) {
+    if (c.taps.empty() || c.ecount == 0) { fe->tap_read_pre = false; return 0; }
+    c.tap_off.assign(c.taps.size(), 0);
+    size_t need = 0, need_max = 0;
+    for (size_t k = 0; k < c.taps.size(); k++) {
+        if (c.kernel_out[c.taps[k]]) { continue; }
+        const size_t b = iq_tap_bytes(fe->vfos[c.taps[k]]->tap_type);
+        c.tap_off[k] = need;
+        need += ((size_t)c.ecount * b + 15) & ~(size_t)15;
+        need_max += ((size_t)fe->max_eff * b + 15) & ~(size_t)15;
+    }
+    int rc;
+    if (fe->tap_stage[c.slot].bytes < need && (rc = fe->tap_stage[c.slot].alloc(need_max, false))) { return rc; }
+    B200_CK(cudaEventRecord(fe->ev_tap_go, fe->sch.stream));
+    B200_CK(cudaStreamWaitEvent(fe->tap_stream, fe->ev_tap_go, 0));
+    cudaEvent_t t_tap = fe->sch.timer_begin(3, fe->tap_stream);
+    IqTapParams tp;
+    memset(&tp, 0, sizeof(tp));
+    tp.in = c.ein; tp.fmt = c.efmt; tp.n = c.ecount; tp.in_scale = c.escale;
+    auto aligned = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+    for (size_t k0 = 0; k0 < c.taps.size(); k0 += IQT_MAX) {
+        tp.njobs = 0;
+        tp.vec = aligned(c.ein) ? 1 : 0;
+        for (size_t k = k0; k < c.taps.size() && k < k0 + IQT_MAX; k++) {
+            const VfoSlot* v = fe->vfos[c.taps[k]].get();
+            void* dst = c.kernel_out[c.taps[k]] ? c.out->vfo_out[c.taps[k]] : (void*)((char*)fe->tap_stage[c.slot].p + c.tap_off[k]);
+            tp.job[tp.njobs++] = IqTapJob{ dst, v->tap_type, v->tap_scalar };
+            tp.vec &= aligned(dst) ? 1 : 0;
+        }
+        cudaError_t e = launch_iq_tap(tp, fe->tap_stream);
+        if (e != cudaSuccess) { return cuda_fail(e, "launch_iq_tap"); }
+        fe->sch.launches++;
+    }
+    if (t_tap) { B200_CK(cudaEventRecord(t_tap, fe->tap_stream)); }
+    B200_CK(cudaEventRecord(fe->ev_tap_done, fe->tap_stream));
+    c.tap_forked = true;
+    fe->tap_read_pre = fe->decim > 1 && !fe->dc_block && !fe->invert_iq;
+    return 0;
+}
+
+// The spectrum branch (IQFrontEnd's Reshaper -> FFT): the frames of the effective stream, nz samples every nz + skip, on
+// fft_stream.  It only reads the chunk, so it forks from the main stream at its first enqueue, runs beside the VFO branch
+// and joins before the outputs.
+static int fe_fft_chunk(b200_fe* fe, FeChunk& c) {
+    if (!fe->fft_on) { fe->pos += (unsigned long long)c.ecount; return 0; }
+    const int bps = bytes_per_sample(c.efmt);
+    const unsigned long long pos = fe->pos, end = pos + (unsigned long long)c.ecount;
+    const unsigned long long nz = (unsigned long long)fe->fft.nz, interval = nz + (unsigned long long)fe->skip;
+    fe->fft.plan.in_scale = c.escale;
+    float* const lines_base = c.direct ? c.out->fft_out : fe->lines.as<float>();
+    cudaStream_t s = fe->fft_stream;
     cudaEvent_t t_fft = nullptr;
     auto fork = [&]() -> int {
-        // the spectrum branch only reads the chunk: run it beside the VFO branch, join before the outputs
-        if (async && !forked) {
-            B200_CK(cudaEventRecord(fe->ev_fft_go, main_s));
-            B200_CK(cudaStreamWaitEvent(s, fe->ev_fft_go, 0));
-            // the line buffer of the previous chunk may still be on its way out (tail stream)
-            if (fe->lines_busy) { B200_CK(cudaStreamWaitEvent(s, fe->ev_lines_free, 0)); }
-            trace_mark("fft start", s);
-            t_fft = fe->sch.timer_begin(2, s);
-            forked = true;
-        }
+        if (c.fft_forked) { return 0; }
+        B200_CK(cudaEventRecord(fe->ev_fft_go, fe->sch.stream));
+        B200_CK(cudaStreamWaitEvent(s, fe->ev_fft_go, 0));
+        // the line buffer of the previous chunk may still be on its way out (tail stream)
+        if (fe->lines_busy) { B200_CK(cudaStreamWaitEvent(s, fe->ev_lines_free, 0)); }
+        trace_mark("fft start", s);
+        t_fft = fe->sch.timer_begin(2, s);
+        c.fft_forked = true;
         return 0;
     };
     int rc = 0;
     char* const frame = (char*)fe->frame.p;
-    // a frame begun in earlier chunks whose staged part this chunk cannot extend in place (other format or scale, or the
-    // cf32 staging of fft_v 0): convert that part to cf32 through the work buffer, and carry the frame on in cf32
     const bool pending = fe->fstart < pos;
-    const bool same_fmt = fe->frame_fmt == fmt && (fmt == FMT_CF32 || fe->frame_scale == isc);
-    if (pending && (!fe->fft_v || !same_fmt) && fe->frame_fmt != FMT_CF32) {
-        if ((rc = fork())) { return rc; }
-        const int len = (int)(pos - fe->fstart);
-        cudaError_t e = launch_convert_cf32(frame, fe->frame_fmt, fe->fft.work.as<float2>(), len, fe->frame_scale, s);
-        if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
-        fe->sch.launches++;
-        B200_CK(cudaMemcpyAsync(frame, fe->fft.work.p, (size_t)len * sizeof(float2), cudaMemcpyDeviceToDevice, s));
-        fe->frame_fmt = FMT_CF32;
-        fe->frame_scale = 0.0f;
-    }
+    const bool same_fmt = fe->frame_fmt == c.efmt && (c.efmt == FMT_CF32 || fe->frame_scale == c.escale);
     if (pending && (!fe->fft_v || !same_fmt)) {
+        // a frame begun in earlier chunks whose staged part this chunk cannot extend in place (other format or scale, or the
+        // cf32 staging of fft_v 0): convert that part to cf32 through the work buffer, and carry the frame on in cf32
+        if (fe->frame_fmt != FMT_CF32) {
+            if ((rc = fork())) { return rc; }
+            const int len = (int)(pos - fe->fstart);
+            cudaError_t e = launch_convert_cf32(frame, fe->frame_fmt, fe->fft.work.as<float2>(), len, fe->frame_scale, s);
+            if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
+            fe->sch.launches++;
+            B200_CK(cudaMemcpyAsync(frame, fe->fft.work.p, (size_t)len * sizeof(float2), cudaMemcpyDeviceToDevice, s));
+            fe->frame_fmt = FMT_CF32;
+            fe->frame_scale = 0.0f;
+        }
         // 1) this chunk's part of the frame, converted behind the staged cf32 part; transformed alone if it completes here
         const unsigned long long fend = fe->fstart + nz;
         const unsigned long long lo = pos, hi = std::min(fend, end);
         if (hi > lo) {
             if ((rc = fork())) { return rc; }
-            cudaError_t e = launch_convert_cf32(dptr, fmt, fe->frame.as<float2>() + (size_t)(lo - fe->fstart), (int)(hi - lo), isc, s);
+            cudaError_t e = launch_convert_cf32(c.ein, c.efmt, fe->frame.as<float2>() + (size_t)(lo - fe->fstart), (int)(hi - lo), c.escale, s);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
             fe->sch.launches++;
         }
@@ -1152,321 +1300,177 @@ static int fe_fft_chunk(b200_fe* fe, const void* dptr, int fmt, int count, int* 
             cudaError_t e = launch_fft_frames(fe->fft.plan, fr, FMT_CF32, fe->fft.work.as<float2>(), lines_base, nullptr, s, &nl, fe->fft_v != 0);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_fft_frames"); }
             fe->sch.launches += nl;
-            (*nlines)++;
+            c.nlines++;
             fe->fstart += interval;
         }
     }
     else if (pending && fe->fstart + nz > end) {
         // a frame that spans this whole chunk: append the chunk to its staged part
-        if (count > 0) {
+        if (c.ecount > 0) {
             if ((rc = fork())) { return rc; }
-            B200_CK(cudaMemcpyAsync(frame + (size_t)(pos - fe->fstart) * bps, dptr, (size_t)count * bps, cudaMemcpyDeviceToDevice, s));
+            B200_CK(cudaMemcpyAsync(frame + (size_t)(pos - fe->fstart) * bps, c.ein, (size_t)c.ecount * bps, cudaMemcpyDeviceToDevice, s));
         }
     }
     // 2) the frames that complete in this chunk, one batched launch pair.  With fft_v 1 the first may have begun in earlier
     // chunks: its first `split` samples come from the staged part, the rest straight from the chunk.
     const unsigned long long split = fe->fstart < pos ? pos - fe->fstart : 0;
-    if (fe->fstart + nz <= end) {
-        int nb = (int)((end - fe->fstart - nz) / interval) + 1;
-        if (*nlines + nb > fe->max_lines) { set_error("FFT line buffer overflow"); return B200_ECAP; }
+    const int nb = fft_frames_by(fe, end);
+    if (nb > 0) {
         if ((rc = fork())) { return rc; }
-        const FftFrames fr{ (const char*)dptr + (size_t)(fe->fstart + split - pos) * bps, frame, (long long)interval, (int)split, nb };
+        const FftFrames fr{ (const char*)c.ein + (size_t)(fe->fstart + split - pos) * bps, frame, (long long)interval, (int)split, nb };
         int nl = 0;
-        cudaError_t e = launch_fft_frames(fe->fft.plan, fr, fmt, fe->fft.work.as<float2>(), lines_base + (size_t)(*nlines) * fe->fft.size,
+        cudaError_t e = launch_fft_frames(fe->fft.plan, fr, c.efmt, fe->fft.work.as<float2>(), lines_base + (size_t)c.nlines * fe->fft.size,
                                           nullptr, s, &nl, fe->fft_v != 0);
         if (e != cudaSuccess) { return cuda_fail(e, "launch_fft_frames"); }
         fe->sch.launches += nl;
-        *nlines += nb;
+        c.nlines += nb;
         fe->fstart += interval * (unsigned long long)nb;
     }
     // 3) the head of a frame that continues into the next chunk
     if (fe->fstart < end && fe->fstart >= pos) {
         const unsigned long long lo = fe->fstart, hi = end;
         if ((rc = fork())) { return rc; }
-        const char* src = (const char*)dptr + (size_t)(lo - pos) * bps;
+        const char* src = (const char*)c.ein + (size_t)(lo - pos) * bps;
         if (fe->fft_v) {
             B200_CK(cudaMemcpyAsync(frame, src, (size_t)(hi - lo) * bps, cudaMemcpyDeviceToDevice, s));
-            fe->frame_fmt = fmt;
-            fe->frame_scale = isc;
+            fe->frame_fmt = c.efmt;
+            fe->frame_scale = c.escale;
         }
         else {
-            cudaError_t e = launch_convert_cf32(src, fmt, fe->frame.as<float2>(), (int)(hi - lo), isc, s);
+            cudaError_t e = launch_convert_cf32(src, c.efmt, fe->frame.as<float2>(), (int)(hi - lo), c.escale, s);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
             fe->sch.launches++;
             fe->frame_fmt = FMT_CF32;
             fe->frame_scale = 0.0f;
         }
     }
-    if (forked) {
+    if (c.fft_forked) {
         if (t_fft) { B200_CK(cudaEventRecord(t_fft, s)); }
         trace_mark("fft done", s);
         B200_CK(cudaEventRecord(fe->ev_fft_done, s));
-        fe->fft_join_pending = true;     // joined by the caller after the VFO branch has been enqueued
-        // stage 1 of this chunk behind its spectrum branch: the two read the same chunk and, run side by side, slow each other
-        // down by more than running one after the other costs; the chain behind stage 1 (its own stream) fills the SMs beside them
-        if (fe->fft_serial && s != main_s) { B200_CK(cudaStreamWaitEvent(main_s, fe->ev_fft_done, 0)); }
     }
     fe->pos = end;
     return 0;
 }
 
-extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt, int in_mem, b200_outputs* out) {
-    if (!fe || !out || (count > 0 && !iq)) { set_error("null argument"); return B200_EINVAL; }
-    if (count < 0 || count > fe->max_chunk) { set_error("count %d exceeds max_chunk %d", count, fe->max_chunk); return B200_ECAP; }
-    if (in_fmt < 0 || in_fmt > 2) { set_error("bad input format"); return B200_EINVAL; }
-    if (fe->nsub - fe->nwait >= (unsigned long long)fe->max_inflight) { set_error("%d chunks already in flight: call b200_fe_wait", fe->max_inflight); return B200_ESTATE; }
-    std::lock_guard<std::mutex> lck(fe->mtx);
-    const long long hp0 = host_clock_ns();
-    { int rcp = apply_pending(fe); if (rcp) { return rcp; } }
-    const int slot = (int)(fe->nsub % FE_SLOTS);
-    cudaStream_t s = fe->sch.stream;
-    const size_t in_bytes = (size_t)count * bytes_per_sample(in_fmt);
-    // ---- capacity checks against the exact counts, before anything is enqueued and before any state moves ----
-    std::vector<Chain*> chains;
-    std::vector<int> ids, taps;
-    for (size_t i = 0; i < fe->vfos.size(); i++) {
-        const VfoSlot* v = fe->vfos[i].get();
-        if (!v->used || is_rds_out(v)) { continue; }
-        if (is_tap(v)) { taps.push_back((int)i); continue; }
-        chains.push_back(&fe->vfos[i]->chain); ids.push_back((int)i);
-        // a bound RDS branch right behind the VFO whose discriminator feeds it (Chain::parent)
-        if (v->rds_child >= 0) { chains.push_back(&fe->vfos[v->rds_child]->chain); ids.push_back(v->rds_child); }
-    }
-    // samples that reach the FFT branch and the VFOs: the chunk itself, or what the input decimator makes of it
-    const int ecount = (fe->decim > 1) ? fe->pre.peek(count) : count;
-    if (ecount < 0) { set_error("input decimator is not a FIR cascade"); return B200_ESTATE; }
-    for (size_t k = 0; k < chains.size(); k++) {
-        int bound = vfo_out_bound(fe, fe->vfos[ids[k]].get(), ecount);
-        if (out->vfo_out[ids[k]] == nullptr || out->vfo_cap[ids[k]] < bound) {
-            set_error("VFO %d output buffer too small: need room for %d samples (b200_fe_vfo_max_out)", ids[k], bound);
-            return B200_ECAP;
-        }
-    }
-    for (int id : taps) {
-        if (out->vfo_out[id] == nullptr || out->vfo_cap[id] < ecount) {
-            set_error("IQ tap %d output buffer too small: need room for %d samples (b200_fe_vfo_max_out)", id, ecount);
-            return B200_ECAP;
-        }
-    }
-    if (fe->fft_on) {
-        // exact count of lines this chunk completes
-        unsigned long long end = fe->pos + (unsigned long long)ecount, f = fe->fstart;
-        unsigned long long nz = (unsigned long long)fe->fft.nz, iv = nz + (unsigned long long)fe->skip;
-        int need = 0;
-        while (f + nz <= end) { need++; f += iv; }
-        if (need > fe->max_lines) { set_error("FFT line buffer overflow: %d lines complete in this chunk, room for %d", need, fe->max_lines); return B200_ECAP; }
-        if (need > 0 && (out->fft_out == nullptr || out->fft_cap_lines < need)) {
-            set_error("FFT output buffer too small: %d lines complete in this chunk", need);
-            return B200_ECAP;
-        }
-    }
-    const void* dptr = iq;
-    if (in_mem == B200_MEM_HOST && count > 0) {
-        if (fe->in_dev[slot].bytes < in_bytes) {
-            B200_CK(cudaStreamSynchronize(s));
-            int rc = fe->in_dev[slot].alloc(std::max(in_bytes, (size_t)fe->max_chunk * bytes_per_sample(in_fmt)), false);
-            if (rc) { return rc; }
-        }
-        if (fe->slot_used[slot]) { B200_CK(cudaStreamWaitEvent(fe->copy_stream, fe->ev_compute[slot], 0)); }
-        trace_mark("h2d start", fe->copy_stream);
-        B200_CK(cudaMemcpyAsync(fe->in_dev[slot].p, iq, in_bytes, cudaMemcpyHostToDevice, fe->copy_stream));
-        trace_mark("h2d done", fe->copy_stream);
-        B200_CK(cudaEventRecord(fe->ev_h2d[slot], fe->copy_stream));
-        B200_CK(cudaStreamWaitEvent(s, fe->ev_h2d[slot], 0));
-        dptr = fe->in_dev[slot].p;
-    }
-    { int rcd = fe->sch.apply_deferred(chains); if (rcd) { return rcd; } }
-    // ---- IQFrontEnd pre-processing chain (iq_frontend.cpp:32-39): decimator -> DC blocker -> conjugate ----
-    if (fe->decim > 1 || fe->dc_block || fe->invert_iq) {
-        if (fe->slot_used[slot]) { B200_CK(cudaStreamWaitEvent(s, fe->ev_compute[slot], 0)); }     // pp[slot] of two chunks ago
-        const void* cur = dptr;
-        int cur_fmt = in_fmt;
-        if (fe->decim > 1) {
-            // the decimator's output is one buffer: the last chunk's IQ taps may still be reading it
-            if (fe->tap_read_pre) { B200_CK(cudaStreamWaitEvent(s, fe->ev_tap_done, 0)); }
-            cudaError_t e = launch_convert_cf32(dptr, in_fmt, (float2*)fe->pre.st[0]->in_data(), count, fe_ingest_scale(fe, in_fmt), s);
-            if (e != cudaSuccess) { return cuda_fail(e, "launch_convert_cf32"); }
-            fe->sch.launches++;
-            fe->pre.plan(count);
-            std::vector<Chain*> pc{ &fe->pre };
-            const long long l0 = fe->sch_pre.launches;
-            fe->sch_pre.stream = s;
-            int rcp = fe->sch_pre.run(pc, nullptr, FMT_CF32, count, false);
-            if (rcp) { return rcp; }
-            fe->sch.launches += fe->sch_pre.launches - l0;
-            cur = fe->pre.out.p;
-            cur_fmt = FMT_CF32;
-        }
-        if (fe->dc_block || fe->invert_iq) {
-            const size_t need = ((size_t)fe->max_eff + 8) * sizeof(float2);
-            if (fe->pp[slot].bytes < need) { int rca = fe->pp[slot].alloc(need, false); if (rca) { return rca; } }
-            const int nseg_max = fe->max_eff / 4096 + 2;
-            if (!fe->dc_state.p) {
-                int rca;
-                if ((rca = fe->dc_state.alloc(16)) || (rca = fe->dc_segA.alloc((size_t)nseg_max * sizeof(float), false)) ||
-                    (rca = fe->dc_segB.alloc((size_t)nseg_max * sizeof(float2), false))) { return rca; }
-            }
-            DcbParams dp;
-            memset(&dp, 0, sizeof(dp));
-            dp.in = cur; dp.out = fe->pp[slot].as<float2>(); dp.fmt = cur_fmt; dp.count = ecount;
-            dp.in_scale = fe_ingest_scale(fe, cur_fmt);
-            dp.rate = (float)(50.0 / fe->fs_eff);                      // genDCBlockRate (iq_frontend.h:55-57)
-            dp.dc_on = fe->dc_block ? 1 : 0; dp.conj_on = fe->invert_iq ? 1 : 0;
-            dp.state = fe->dc_state.as<float2>(); dp.segA = fe->dc_segA.as<float>(); dp.segB = fe->dc_segB.as<float2>();
-            dp.nseg = (ecount + 4095) / 4096;
-            int nl = 0;
-            cudaError_t e = launch_preproc(dp, s, &nl);
-            if (e != cudaSuccess) { return cuda_fail(e, "launch_preproc"); }
-            fe->sch.launches += nl;
-            cur = fe->pp[slot].p;
-            cur_fmt = FMT_CF32;
-        }
-        dptr = cur;
-        in_fmt = cur_fmt;
-        count = ecount;
-    }
-    for (Chain* c : chains) { c->plan(c->parent ? c->parent->st[c->parent->quad_index()]->n_out : count); }
-    // device-resident outputs: the last stage of every chain (and the FFT epilogue) write straight into the caller's buffers
-    const bool direct = (out->out_mem == B200_MEM_DEVICE);
-    // host outputs of a small chunk: the last kernel of a VFO stores straight into the caller's pinned buffer (a few KB over
-    // PCIe) when that buffer came from b200_host_alloc; large chunks keep the copy engine
-    const bool host_direct = !direct && fe->host_direct != 0 && (fe->host_direct > 0 || count <= (1 << 22));
-    std::vector<char> vdirect(chains.size(), direct ? 1 : 0);
-    for (size_t k = 0; k < chains.size(); k++) {
-        if (host_direct && host_buffer_is_ours(out->vfo_out[ids[k]], (size_t)out->vfo_cap[ids[k]] * chains[k]->out_es * sizeof(float))) { vdirect[k] = 1; }
-        // an RDS VFO's chain output stays in the chain: RDSDemod reads it there and writes the caller's buffer itself
-        chains[k]->out_override = (vdirect[k] && !fe->vfos[ids[k]]->rds) ? (float*)out->vfo_out[ids[k]] : nullptr;
-    }
-    fe->lines_override = direct ? out->fft_out : nullptr;
-    int nlines = 0;
+// RDSDemod behind the WFM_RDS_BITS VFOs and bound RDS outputs: one launch per B200_BATCH of those with 5 kS/s samples this
+// chunk, on the stream of the tails, behind them and in front of the next chunk's (which overwrite the chain outputs and
+// move the RDS states)
+static int fe_rds(b200_fe* fe, FeChunk& c) {
+    fe->rds_pend[c.slot].clear();
+    fe->rds_out[c.slot] = c.out;
+    if (!fe->rds_count) { return 0; }        // allocated with the first RDS demodulator: a handle that never had one skips all this
+    RdsParams rp;
+    memset(&rp, 0, sizeof(rp));
+    auto flush = [&]() -> int {
+        cudaError_t e = launch_rds_demod(rp, fe->sch.out_stream());
+        if (e != cudaSuccess) { return cuda_fail(e, "launch_rds_demod"); }
+        fe->sch.launches += rp.njobs > 0 ? 1 : 0;
+        rp.njobs = 0;
+        return 0;
+    };
     int rc;
-    // IQ taps: k_iq_tap reads the effective stream once and stores every tap, on its own stream so that neither the VFO
-    // branch nor the spectrum branch waits for it.  A tap writes the caller's buffer itself when that is device memory, or a
-    // b200_host_alloc buffer under the VFOs' rule -- with host_direct -1 only for outputs up to TAP_DIRECT_MAX bytes: the
-    // kernel's own stores over PCIe moved a 1 Mi-sample CF32 tap (8 MiB) at a third of the copy engine's rate.  Otherwise the
-    // tap fills its region of tap_stage[slot], copied out on the join stream.  tap_stage[slot] was last read by the copies of
-    // chunk nsub - FE_SLOTS, which b200_fe_wait has seen complete.
-    const size_t TAP_DIRECT_MAX = 64 << 10;
-    std::vector<size_t> tap_off(taps.size(), SIZE_MAX);
-    bool tap_forked = false;
-    if (!taps.empty() && count > 0) {
-        size_t need = 0, need_max = 0;
-        for (size_t k = 0; k < taps.size(); k++) {
-            const size_t b = iq_tap_bytes(fe->vfos[taps[k]]->tap_type);
-            const bool small = fe->host_direct > 0 || (size_t)count * b <= TAP_DIRECT_MAX;
-            if (direct || (host_direct && small && host_buffer_is_ours(out->vfo_out[taps[k]], (size_t)out->vfo_cap[taps[k]] * b))) { continue; }
-            tap_off[k] = need;
-            need += ((size_t)count * b + 15) & ~(size_t)15;
-            need_max += ((size_t)fe->max_eff * b + 15) & ~(size_t)15;
-        }
-        if (fe->tap_stage[slot].bytes < need && (rc = fe->tap_stage[slot].alloc(need_max, false))) { return rc; }
-        B200_CK(cudaEventRecord(fe->ev_tap_go, s));
-        B200_CK(cudaStreamWaitEvent(fe->tap_stream, fe->ev_tap_go, 0));
-        cudaEvent_t t_tap = fe->sch.timer_begin(3, fe->tap_stream);
-        IqTapParams tp;
-        memset(&tp, 0, sizeof(tp));
-        tp.in = dptr; tp.fmt = in_fmt; tp.n = count; tp.in_scale = fe_ingest_scale(fe, in_fmt);
-        auto aligned = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
-        for (size_t k0 = 0; k0 < taps.size(); k0 += IQT_MAX) {
-            tp.njobs = 0;
-            tp.vec = aligned(dptr) ? 1 : 0;
-            for (size_t k = k0; k < taps.size() && k < k0 + IQT_MAX; k++) {
-                const VfoSlot* v = fe->vfos[taps[k]].get();
-                void* dst = tap_off[k] == SIZE_MAX ? out->vfo_out[taps[k]] : (void*)((char*)fe->tap_stage[slot].p + tap_off[k]);
-                tp.job[tp.njobs++] = IqTapJob{ dst, v->tap_type, v->tap_scalar };
-                tp.vec &= aligned(dst) ? 1 : 0;
-            }
-            cudaError_t e = launch_iq_tap(tp, fe->tap_stream);
-            if (e != cudaSuccess) { return cuda_fail(e, "launch_iq_tap"); }
-            fe->sch.launches++;
-        }
-        if (t_tap) { B200_CK(cudaEventRecord(t_tap, fe->tap_stream)); }
-        B200_CK(cudaEventRecord(fe->ev_tap_done, fe->tap_stream));
-        tap_forked = true;
+    for (size_t k = 0; k < c.chains.size(); k++) {
+        const int id = c.ids[k];
+        VfoSlot* v = fe->vfos[id].get();
+        if (!v->rds) { continue; }
+        const int n = c.chains[k]->n_out, bound = b200_rds_demod_max_out(n);
+        fe->rds_pend[c.slot].push_back({ id, n, bound });
+        if (n == 0) { continue; }
+        RdsSym* dst = c.kernel_out[id] ? (RdsSym*)c.out->vfo_out[id] : v->rds_rec.as<RdsSym>();
+        rp.job[rp.njobs++] = v->rds->job(c.chains[k]->out.as<float2>(), n, dst, bound, fe->rds_count + c.slot * B200_MAX_VFOS + id);
+        if (rp.njobs == B200_BATCH && (rc = flush())) { return rc; }
     }
-    fe->tap_read_pre = tap_forked && fe->decim > 1 && !fe->dc_block && !fe->invert_iq;
-    // fork the spectrum branch first; its join (a wait on the main stream) comes after the VFO branch has been
-    // enqueued, so the two overlap on the device
-    const long long hp1 = host_clock_ns();
-    if ((rc = fe_fft_chunk(fe, dptr, in_fmt, count, &nlines))) { return rc; }
-    const long long hp2 = host_clock_ns();
-    fe->sch.in_scale = fe_ingest_scale(fe, in_fmt);
-    // host-side outputs leave through per-VFO device buffers that the copies of the previous chunk may still be reading
-    if (!direct && fe->nsub > 0) { B200_CK(cudaStreamWaitEvent(fe->sch.out_stream(), fe->ev_out[(slot + FE_SLOTS - 1) % FE_SLOTS], 0)); }
-    if ((rc = fe->sch.run(chains, dptr, in_fmt, count, true))) { return rc; }
-    // RDSDemod behind the WFM_RDS_BITS VFOs: one launch per B200_BATCH of those with 5 kS/s samples this chunk, on the stream of
-    // the tails, behind them and in front of the next chunk's (which overwrite the chain outputs and move the RDS states)
-    fe->rds_pend[slot].clear();
-    fe->rds_out[slot] = out;
-    if (fe->rds_count) {         // allocated with the first WFM_RDS_BITS VFO: a handle that never had one skips all this
-        RdsParams rp;
-        memset(&rp, 0, sizeof(rp));
-        auto flush = [&]() -> int {
-            cudaError_t e = launch_rds_demod(rp, fe->sch.out_stream());
-            if (e != cudaSuccess) { return cuda_fail(e, "launch_rds_demod"); }
-            fe->sch.launches += rp.njobs > 0 ? 1 : 0;
-            rp.njobs = 0;
-            return 0;
-        };
-        for (size_t k = 0; k < chains.size(); k++) {
-            VfoSlot* v = fe->vfos[ids[k]].get();
-            if (!v->rds) { continue; }
-            const int n = chains[k]->n_out, bound = b200_rds_demod_max_out(n);
-            fe->rds_pend[slot].push_back({ ids[k], n, bound });
-            if (n == 0) { continue; }
-            RdsSym* dst = vdirect[k] ? (RdsSym*)out->vfo_out[ids[k]] : v->rds_rec.as<RdsSym>();
-            rp.job[rp.njobs++] = v->rds->job(chains[k]->out.as<float2>(), n, dst, bound, fe->rds_count + slot * B200_MAX_VFOS + ids[k]);
-            if (rp.njobs == B200_BATCH && (rc = flush())) { return rc; }
-        }
-        if ((rc = flush())) { return rc; }
-    }
-    const long long hp3 = host_clock_ns();
-    // join on a stream of its own: the VFO branch (tail stream) and the spectrum branch (its stream) of this chunk meet
-    // here, neither waits for the other -- the tail stream goes straight on to the next chunk
+    return flush();
+}
+
+// The join on a stream of its own: the VFO branch (tail stream), the spectrum branch and the IQ taps (their streams) of this
+// chunk meet here, and none waits for another -- the tail stream goes straight on to the next chunk.  Then every output that
+// no kernel wrote into the caller's buffer is copied there.
+static int fe_join_and_copy_out(b200_fe* fe, FeChunk& c) {
+    b200_outputs* out = c.out;
     cudaStream_t os = fe->join_stream;
-    B200_CK(cudaEventRecord(fe->ev_tail_done[slot], fe->sch.out_stream()));
-    B200_CK(cudaStreamWaitEvent(os, fe->ev_tail_done[slot], 0));
-    if (fe->fft_join_pending) {
-        B200_CK(cudaStreamWaitEvent(os, fe->ev_fft_done, 0));
-        fe->fft_join_pending = false;
-    }
-    if (tap_forked) { B200_CK(cudaStreamWaitEvent(os, fe->ev_tap_done, 0)); }
+    B200_CK(cudaEventRecord(fe->ev_tail_done[c.slot], fe->sch.out_stream()));
+    B200_CK(cudaStreamWaitEvent(os, fe->ev_tail_done[c.slot], 0));
+    if (c.fft_forked) { B200_CK(cudaStreamWaitEvent(os, fe->ev_fft_done, 0)); }
+    if (c.tap_forked) { B200_CK(cudaStreamWaitEvent(os, fe->ev_tap_done, 0)); }
     // the input chunk is no longer needed once stage 1, the raw carry (both in front of the tail on its stream) and the
     // spectrum branch are done
-    B200_CK(cudaEventRecord(fe->ev_compute[slot], os));
-    fe->slot_used[slot] = true;
-    // ---- outputs ----
-    const cudaMemcpyKind kind = (out->out_mem == B200_MEM_DEVICE) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    for (size_t k = 0; k < chains.size(); k++) {
-        Chain* c = chains[k];
-        if (fe->vfos[ids[k]]->rds) {
+    B200_CK(cudaEventRecord(fe->ev_compute[c.slot], os));
+    fe->slot_used[c.slot] = true;
+    const cudaMemcpyKind kind = c.direct ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    for (size_t k = 0; k < c.chains.size(); k++) {
+        const Chain* ch = c.chains[k];
+        const int id = c.ids[k];
+        if (fe->vfos[id]->rds) {
             // the symbol count is known after the launch: every record the bound allows leaves, b200_fe_wait sets the count
-            const int bound = b200_rds_demod_max_out(c->n_out);
-            if (c->n_out > 0 && !vdirect[k]) {
-                B200_CK(cudaMemcpyAsync(out->vfo_out[ids[k]], fe->vfos[ids[k]]->rds_rec.p, (size_t)bound * sizeof(RdsSym), kind, os));
+            const int bound = b200_rds_demod_max_out(ch->n_out);
+            if (ch->n_out > 0 && !c.kernel_out[id]) {
+                B200_CK(cudaMemcpyAsync(out->vfo_out[id], fe->vfos[id]->rds_rec.p, (size_t)bound * sizeof(RdsSym), kind, os));
             }
             continue;
         }
-        out->vfo_count[ids[k]] = c->n_out;
-        if (c->n_out > 0 && !vdirect[k]) {
-            B200_CK(cudaMemcpyAsync(out->vfo_out[ids[k]], c->out.p, (size_t)c->n_out * c->out_es * sizeof(float), kind, os));
+        out->vfo_count[id] = ch->n_out;
+        if (ch->n_out > 0 && !c.kernel_out[id]) {
+            B200_CK(cudaMemcpyAsync(out->vfo_out[id], ch->out.p, (size_t)ch->n_out * ch->out_es * sizeof(float), kind, os));
         }
     }
-    for (size_t k = 0; k < taps.size(); k++) {
-        out->vfo_count[taps[k]] = count;
-        if (count > 0 && tap_off[k] != SIZE_MAX) {
-            B200_CK(cudaMemcpyAsync(out->vfo_out[taps[k]], (const char*)fe->tap_stage[slot].p + tap_off[k],
-                                    (size_t)count * iq_tap_bytes(fe->vfos[taps[k]]->tap_type), kind, os));
+    for (size_t k = 0; k < c.taps.size(); k++) {
+        const int id = c.taps[k];
+        out->vfo_count[id] = c.ecount;
+        if (c.ecount > 0 && !c.kernel_out[id]) {
+            B200_CK(cudaMemcpyAsync(out->vfo_out[id], (const char*)fe->tap_stage[c.slot].p + c.tap_off[k],
+                                    (size_t)c.ecount * iq_tap_bytes(fe->vfos[id]->tap_type), kind, os));
         }
     }
-    out->fft_lines = nlines;
-    if (nlines > 0 && !direct) {
-        B200_CK(cudaMemcpyAsync(out->fft_out, fe->lines.p, (size_t)nlines * fe->fft.size * sizeof(float), kind, os));
+    out->fft_lines = c.nlines;
+    if (c.nlines > 0 && !c.direct) {
+        B200_CK(cudaMemcpyAsync(out->fft_out, fe->lines.p, (size_t)c.nlines * fe->fft.size * sizeof(float), kind, os));
         B200_CK(cudaEventRecord(fe->ev_lines_free, os));
         fe->lines_busy = true;
     }
-    B200_CK(cudaEventRecord(fe->ev_out[slot], os));
+    B200_CK(cudaEventRecord(fe->ev_out[c.slot], os));
     trace_mark("outputs done", os);
+    return 0;
+}
+
+// what b200_fe_submit and b200_shard_submit check of a chunk before anything else
+static int check_chunk_args(const b200_fe* fe, int count, int in_fmt, const b200_outputs* out) {
+    if (!out) { set_error("null argument"); return B200_EINVAL; }
+    if (count < 0 || count > fe->max_chunk) { set_error("count %d exceeds max_chunk %d", count, fe->max_chunk); return B200_ECAP; }
+    if (in_fmt < 0 || in_fmt > 2) { set_error("bad input format"); return B200_EINVAL; }
+    return 0;
+}
+
+extern "C" int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt, int in_mem, b200_outputs* out) {
+    if (!fe || (count > 0 && !iq)) { set_error("null argument"); return B200_EINVAL; }
+    int rc = check_chunk_args(fe, count, in_fmt, out);
+    if (rc) { return rc; }
+    if (fe->nsub - fe->nwait >= (unsigned long long)fe->max_inflight) { set_error("%d chunks already in flight: call b200_fe_wait", fe->max_inflight); return B200_ESTATE; }
+    std::lock_guard<std::mutex> lck(fe->mtx);
+    const long long hp0 = host_clock_ns();
+    if ((rc = apply_pending(fe))) { return rc; }
+    FeChunk c;
+    c.slot = (int)(fe->nsub % FE_SLOTS);
+    c.out = out;
+    c.fmt = in_fmt; c.count = count;
+    // 1/32768 and 1/128 unless the caller set the scale of a compressed-stream packet (b200_fe_set_ingest_scale)
+    c.scale = in_fmt == B200_FMT_CS16 ? fe->scale16 : (in_fmt == B200_FMT_CS8 ? fe->scale8 : 0.0f);
+    c.direct = out->out_mem == B200_MEM_DEVICE;
+    fe_branches(fe, c);
+    if ((rc = fe_check_outputs(fe, c)) || (rc = fe_upload(fe, c, iq, in_mem)) || (rc = fe_preprocess(fe, c))) { return rc; }
+    fe_route_outputs(fe, c);
+    if ((rc = fe_iq_taps(fe, c))) { return rc; }
+    // the spectrum branch forks first; its join comes after the VFO branch has been enqueued, so the two overlap on the device
+    const long long hp1 = host_clock_ns();
+    if ((rc = fe_fft_chunk(fe, c))) { return rc; }
+    const long long hp2 = host_clock_ns();
+    fe->sch.in_scale = c.escale;
+    // host-side outputs leave through per-VFO device buffers that the copies of the previous chunk may still be reading
+    if (!c.direct && fe->nsub > 0) { B200_CK(cudaStreamWaitEvent(fe->sch.out_stream(), fe->ev_out[(c.slot + FE_SLOTS - 1) % FE_SLOTS], 0)); }
+    if ((rc = fe->sch.run(c.chains, c.ein, c.efmt, c.ecount, true)) || (rc = fe_rds(fe, c))) { return rc; }
+    const long long hp3 = host_clock_ns();
+    if ((rc = fe_join_and_copy_out(fe, c))) { return rc; }
     fe->nsub++;
     const long long hp4 = host_clock_ns();
     fe->host_ns[0] += hp1 - hp0; fe->host_ns[1] += hp2 - hp1; fe->host_ns[2] += hp3 - hp2; fe->host_ns[3] += hp4 - hp3;
@@ -2156,24 +2160,22 @@ extern "C" b200_shard* b200_shard_create(b200_fe* fe, int rank, int world, const
 // Every rank calls submit with the same count and format; `iq` is read on rank 0 only.  Values and counts per VFO are
 // those of b200_fe_submit on the rank that owns the VFO.
 extern "C" int b200_shard_submit(b200_shard* sh, const void* iq, int count, int in_fmt, int in_mem, b200_outputs* out) {
-    if (!sh || !out) { set_error("null argument"); return B200_EINVAL; }
+    if (!sh) { set_error("null argument"); return B200_EINVAL; }
     b200_fe* fe = sh->fe;
-    if (count < 0 || count > fe->max_chunk) { set_error("count %d exceeds max_chunk %d", count, fe->max_chunk); return B200_ECAP; }
-    if (in_fmt < 0 || in_fmt > 2) { set_error("bad input format"); return B200_EINVAL; }
+    int rc = check_chunk_args(fe, count, in_fmt, out);
+    if (rc) { return rc; }
     if (sh->rank == 0 && count > 0 && !iq) { set_error("rank 0 needs the chunk"); return B200_EINVAL; }
     if (fe->nsub - fe->nwait >= 2) { set_error("two chunks already in flight: call b200_shard_wait"); return B200_ESTATE; }
     if (sh->world == 1) {                                   // nothing to fan out: the plain front end
-        int rc1 = b200_fe_submit(fe, iq, count, in_fmt, in_mem, out);
-        if (!rc1) { sh->nsub++; }
-        return rc1;
+        if (!(rc = b200_fe_submit(fe, iq, count, in_fmt, in_mem, out))) { sh->nsub++; }
+        return rc;
     }
     const int slot = (int)(fe->nsub % FE_SLOTS);            // the front end's own input slot of this chunk
     const size_t bytes = (size_t)count * bytes_per_sample(in_fmt);
     cudaStream_t cs = sh->comm_stream, ms = fe->sch.stream;
     if (sh->buf[slot].bytes < bytes) {
         B200_CK(cudaDeviceSynchronize());
-        int rc = sh->buf[slot].alloc(std::max(bytes, (size_t)fe->max_chunk * bytes_per_sample(in_fmt)), false);
-        if (rc) { return rc; }
+        if ((rc = sh->buf[slot].alloc(std::max(bytes, (size_t)fe->max_chunk * bytes_per_sample(in_fmt)), false))) { return rc; }
     }
     // buf[slot] was the input of the chunk two submissions ago: its compute has to be over before it is overwritten
     if (fe->slot_used[slot]) { B200_CK(cudaStreamWaitEvent(cs, fe->ev_compute[slot], 0)); }
@@ -2189,16 +2191,13 @@ extern "C" int b200_shard_submit(b200_shard* sh, const void* iq, int count, int 
                 B200_CK(cudaMemcpyAsync(sh->buf[slot].p, iq, bytes, cudaMemcpyDeviceToDevice, cs));
             }
         }
-        if (sh->world > 1) {
-            int r = nccl().Broadcast(sh->buf[slot].p, sh->buf[slot].p, bytes, 1 /* ncclUint8 */, 0, sh->comm, cs);
-            if (r) { return nccl_fail(r, "ncclBroadcast"); }
-            sh->bytes_broadcast += (long long)bytes;
-        }
+        int r = nccl().Broadcast(sh->buf[slot].p, sh->buf[slot].p, bytes, 1 /* ncclUint8 */, 0, sh->comm, cs);
+        if (r) { return nccl_fail(r, "ncclBroadcast"); }
+        sh->bytes_broadcast += (long long)bytes;
     }
     B200_CK(cudaEventRecord(sh->ev_bcast[slot], cs));
     B200_CK(cudaStreamWaitEvent(ms, sh->ev_bcast[slot], 0));
-    int rc = b200_fe_submit(fe, sh->buf[slot].p, count, in_fmt, B200_MEM_DEVICE, out);
-    if (rc) { return rc; }
+    if ((rc = b200_fe_submit(fe, sh->buf[slot].p, count, in_fmt, B200_MEM_DEVICE, out))) { return rc; }
     sh->nsub++;
     return 0;
 }

@@ -860,6 +860,10 @@ int Scheduler::init_raw() {
 Scheduler::~Scheduler() {
     drop_graphs();
     for (Timer& t : timers) { for (cudaEvent_t e : t.ev) { cudaEventDestroy(e); } }
+    for (int i = 0; i < 2; i++) {
+        if (ev_stage1[i]) { cudaEventDestroy(ev_stage1[i]); }
+        if (ev_tail[i]) { cudaEventDestroy(ev_tail[i]); }
+    }
 }
 cudaEvent_t Scheduler::timer_begin(int group, cudaStream_t s) {
     if (!time_s1) { return nullptr; }

@@ -556,17 +556,17 @@ def test_frontend_multi_vfo_100msps(sb, oracle, report):
     fe.close()
 
 
-@pytest.mark.parametrize("variant,fft_async,overlap,pair,tails", [
-    (5, 1, 1, 1, {}), (5, 0, 0, 1, {"ft_regall": 0}), (0, 1, 0, 0, {}), (5, 1, 1, 0, {"tails": 1}), (5, 1, 0, 1, {"tails": 0}),
-    (6, 1, 1, 1, {"tails": 1}), (6, 1, 0, 0, {"ft_regall": 0}), (6, 1, 1, 1, {"ft_regall": 0, "ft_threads": 256}),
-    (6, 1, 1, 1, {"ft_regall": 0, "ft_ob": 301}), (7, 1, 1, 1, {}), (7, 1, 0, 0, {"tails": 1}), (7, 0, 0, 1, {"ft_regall": 0, "ft_direct": 0}),
-    (6, 1, 0, 1, {"ft_regall": 0, "ft_ob": 64, "ft_smem_kb": 48}), (6, 1, 1, 1, {"ft_regall": 0, "ft_obmax": 2500, "ft_smem_kb": 200}),
-    (8, 1, 1, 1, {}), (8, 0, 0, 0, {"tails": 1}), (8, 1, 1, 1, {"ft_prereg": 0}), (7, 1, 0, 1, {"tails": 1, "ft_prereg": 0}),
-    (8, 1, 1, 1, {"ft_regall": 0}), (8, 1, 1, 1, {"ft_regall": 0, "ft_prereg": 1}), (8, 1, 1, 1, {"s1_stages": 3})])
-def test_frontend_variants_100msps(sb, oracle, report, variant, fft_async, overlap, pair, tails):
+@pytest.mark.parametrize("variant,overlap,pair,tails", [
+    (5, 1, 1, {}), (5, 0, 1, {"ft_regall": 0}), (0, 0, 0, {}), (5, 1, 0, {"tails": 1}), (5, 0, 1, {"tails": 0}),
+    (6, 1, 1, {"tails": 1}), (6, 0, 0, {"ft_regall": 0}), (6, 1, 1, {"ft_regall": 0, "ft_threads": 256}),
+    (6, 1, 1, {"ft_regall": 0, "ft_ob": 301}), (7, 1, 1, {}), (7, 0, 0, {"tails": 1}), (7, 0, 1, {"ft_regall": 0, "ft_direct": 0}),
+    (6, 0, 1, {"ft_regall": 0, "ft_ob": 64, "ft_smem_kb": 48}), (6, 1, 1, {"ft_regall": 0, "ft_obmax": 2500, "ft_smem_kb": 200}),
+    (8, 1, 1, {}), (8, 0, 0, {"tails": 1}), (8, 1, 1, {"ft_prereg": 0}), (7, 0, 1, {"tails": 1, "ft_prereg": 0}),
+    (8, 1, 1, {"ft_regall": 0}), (8, 1, 1, {"ft_regall": 0, "ft_prereg": 1}), (8, 1, 1, {"s1_stages": 3})])
+def test_frontend_variants_100msps(sb, oracle, report, variant, overlap, pair, tails):
     """kernel / scheduling A-B on the config-2 geometry (short): every stage-1 kernel (TMA filter bank, cp.async filter
-    bank, per-VFO complex taps single / double buffered, one thread per output), synchronous spectrum branch, tails on the
-    main stream, conjugate-pair sharing off, register-window tails / fused tail (with forced slab sizes) / per-stage tails."""
+    bank, per-VFO complex taps single / double buffered, one thread per output), tails on the main stream,
+    conjugate-pair sharing off, register-window tails / fused tail (with forced slab sizes) / per-stage tails."""
     fs, chunk, nch = 100e6, 1000000, 4
     n = chunk * nch
     offs = [5e6, -5e6, 15e6, -25e6, 35e6, 25e6]
@@ -577,7 +577,6 @@ def test_frontend_variants_100msps(sb, oracle, report, variant, fft_async, overl
     fe.set_option("overlap", overlap)
     fe.set_option("s1", variant)
     fe.set_option("pair", pair)
-    fe.set_option("fft_async", fft_async)
     for k, v in tails.items():
         fe.set_option(k, v)
     fe.set_fft(1 << 18, 200.0, 2)              # 500000-sample interval: frames inside chunks and across them
@@ -594,7 +593,7 @@ def test_frontend_variants_100msps(sb, oracle, report, variant, fft_async, overl
         assert outs[vid].shape == ya.shape
         errs.append(rel_rms(outs[vid][1500:], ya[1500:]))
     tag = "".join("_%s%d" % kv for kv in sorted(tails.items()))
-    report["frontend_s1v%d_fftasync%d_overlap%d_pair%d%s" % (variant, fft_async, overlap, pair, tag)] = {"wfm_audio_rel_rms": errs, "fft_power_rel_max": e_fft}
+    report["frontend_s1v%d_overlap%d_pair%d%s" % (variant, overlap, pair, tag)] = {"wfm_audio_rel_rms": errs, "fft_power_rel_max": e_fft}
     assert e_fft < TOL, e_fft
     assert max(errs) < TOL, errs
     fe.close()
