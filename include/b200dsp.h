@@ -117,6 +117,10 @@ int b200_load_decim_plans(const char* path /* NULL = default */);
 int b200_taps_lowpass(double cutoff, double transWidth, double samplerate, int oddTapCount, float* out, int cap);
 /* dsp::taps::highPass (core/src/dsp/taps/high_pass.h:7-14) */
 int b200_taps_highpass(double cutoff, double transWidth, double samplerate, int oddTapCount, float* out, int cap);
+/* dsp::taps::bandPass<complex_t> (core/src/dsp/taps/band_pass.h:11-26): returns the tap count, writes min(count,cap) taps as
+ * interleaved (re, im) pairs */
+int b200_taps_bandpass(double bandStart, double bandStop, double transWidth, double samplerate, int oddTapCount,
+                       float* out_iq, int cap);
 /* IQFrontEnd::updateFFTPath window (core/src/signal_path/iq_frontend.cpp:281-291): w(i,nz)*(-1)^i */
 int b200_window(int window, int nz, float* out);
 /* IQFrontEnd::genReshapeParams (core/src/signal_path/iq_frontend.h:59-63) */

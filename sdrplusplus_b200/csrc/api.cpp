@@ -70,6 +70,12 @@ extern "C" int b200_taps_highpass(double cutoff, double tw, double sr, int odd, 
     if (out) { memcpy(out, t.data(), sizeof(float) * (size_t)std::min<int>((int)t.size(), cap)); }
     return (int)t.size();
 }
+extern "C" int b200_taps_bandpass(double b0, double b1, double tw, double sr, int odd, float* out_iq, int cap) {
+    std::vector<float> t = bandpass_c_taps(b0, b1, tw, sr, odd != 0);                   // (re, im) pairs
+    const int n = (int)(t.size() / 2);
+    if (out_iq) { memcpy(out_iq, t.data(), 2 * sizeof(float) * (size_t)std::max(0, std::min(n, cap))); }
+    return n;
+}
 extern "C" int b200_window(int window, int nz, float* out) {
     if (nz < 0 || !out) { set_error("bad window args"); return B200_EINVAL; }
     std::vector<float> w = fft_window(window, nz);

@@ -541,6 +541,15 @@ def taps_highpass(cutoff, tw, sr, odd=False):
     return out
 
 
+def taps_bandpass(band_start, band_stop, tw, sr, odd=False):
+    """taps::bandPass<complex_t>: complex64 taps"""
+    l = L.load()
+    n = l.b200_taps_bandpass(band_start, band_stop, tw, sr, int(odd), None, 0)
+    out = np.empty(n, np.complex64)
+    l.b200_taps_bandpass(band_start, band_stop, tw, sr, int(odd), out.ctypes.data, n)
+    return out
+
+
 def window(win, nz):
     l = L.load()
     out = np.empty(nz, np.float32)

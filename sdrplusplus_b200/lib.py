@@ -60,6 +60,7 @@ SIGNATURES = {
     "b200_load_decim_plans": (_i, [C.c_char_p]),
     "b200_taps_lowpass": (_i, [_d, _d, _d, _i, _vp, _i]),
     "b200_taps_highpass": (_i, [_d, _d, _d, _i, _vp, _i]),
+    "b200_taps_bandpass": (_i, [_d, _d, _d, _d, _i, _vp, _i]),
     "b200_window": (_i, [_i, _i, _vp]),
     "b200_fft_frame_params": (_i, [_d, _i, _d, _ip, _ip]),
     "b200_resamp_plan_get": (_i, [_d, _d, C.POINTER(ResampPlan)]),

@@ -56,6 +56,35 @@ def test_highpass_taps_bit_exact(oracle):
     assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
 
 
+BANDPASS_SETS = [(18750.0, 19250.0, 3000.0, 250000.0, True), (18750.0, 19250.0, 3000.0, 200000.0, True),   # stereo pilot
+                 (1000.0, 3000.0, 500.0, 48000.0, False), (1000.0, 3000.0, 500.0, 48000.0, True),          # even count
+                 (0.0, 2375.0, 100.0, 5000.0, False)]                                                     # RDSDemod
+
+
+@pytest.mark.parametrize("args", BANDPASS_SETS)
+def test_bandpass_taps_bit_exact(oracle, args):
+    """taps::bandPass<complex_t>: the pilot filter of BroadcastFM's stereo branch (odd count, centre off zero) at both IF
+    rates, a set whose estimated count is even with and without the odd fix-up, and RDSDemod's zero-centred set"""
+    a = frontend.taps_bandpass(*args)
+    b = oracle.bandpass_c(*args)
+    assert a.dtype == np.complex64 and a.size == b.size > 0
+    assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+    if args[2:4] == (500.0, 48000.0):
+        assert a.size % 2 == int(args[4])                     # the estimate is even: odd=True adds the one tap
+    if args[0] == 18750.0:
+        assert a.size % 2 == 1 and np.abs(a.imag).max() > 0
+
+
+def test_bandpass_taps_cap():
+    L = lib.load()
+    n = L.b200_taps_bandpass(18750.0, 19250.0, 3000.0, 250000.0, 1, None, 0)
+    out = np.full(2 * n, 7.0, np.float32)
+    assert L.b200_taps_bandpass(18750.0, 19250.0, 3000.0, 250000.0, 1, out.ctypes.data, 5) == n == 317
+    full = frontend.taps_bandpass(18750.0, 19250.0, 3000.0, 250000.0, True)
+    assert np.array_equal(out[:10].view(np.uint32), full[:5].view(np.float32).view(np.uint32))
+    assert np.all(out[10:] == 7.0)
+
+
 @pytest.mark.parametrize("win,nz", [(0, 1000), (1, 4097), (2, 65536), (2, 12000)])
 def test_window_bit_exact(oracle, win, nz):
     assert np.array_equal(frontend.window(win, nz).view(np.uint32), oracle.window_buf(win, nz).view(np.uint32))

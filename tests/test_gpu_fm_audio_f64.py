@@ -44,233 +44,15 @@ import numpy as np
 import pytest
 from scipy.signal import lfilter
 
-from f64_ref import (EDGE, PFB_CASES, POLY_REG, REF_FLOOR, TS_TILE, U, cascade_counts, fir_f64, pfb_detect, pfb_eps, poly_f64,
-                     routes_dfir_reg, schedule, stage1_f64, w_u64)
+from f64_ref import (P32, PFB_CASES, POLY_REG, TS_TILE, TWO_P, U, _gate_clean, _ratio_c, audio_lp_taps, cascade_counts,
+                     chan_taps, deemph_coefs, deemph_f64, fir_f64, inv_dev_of, pfb_detect, poly_f64, quad_f64, quad_ratio,
+                     routes_dfir_reg, schedule, vfo_audio_f64, vfo_counts, volume_f64, w_u64)
 from util import noise_iq
 
-P32 = float(np.float32(3.1415926535))          # FL_M_PI_REF (kernels.cu, oracle/sdrpp_oracle.c FL_M_PI)
-TWO_P = 2.0 * P32                              # 2.0f * FL_M_PI_REF, exact
-ATAN2_ULP = 3
 TAIL_MAX_TAPS = 1024                           # tails.cuh
 FT_MAX_L = 64                                  # fused_tail.cuh
 FT_MAXST = 8                                   # kernels.cuh
 QUAD_TILE = 256                                # k_quad / k_firr_reg outputs per CTA
-
-
-# ---------------------------------------------------------------------------------------------- float64 references
-def ulp32(v):
-    """fp32 ulp of a value of magnitude up to v (a hair above v, so a result that rounds up to the next binade is covered)"""
-    v = np.maximum(np.asarray(v, np.float64) * (1.0 + 2.0 ** -20), 2.0 ** -126)
-    return np.exp2(np.floor(np.log2(v)) - 23.0)
-
-
-def inv_dev_of(dev, sr):
-    """QuadStage::configure / quad_init: (float)(1.0 / hz_to_rads(dev, sr))"""
-    return float(np.float32(1.0 / (2.0 * math.pi * (dev / sr))))
-
-
-def quad_f64(z, b, inv_dev, angles32=False):
-    """discriminator reference and bound (module docstring).  z: IQ (float64 or exact fp32), b: per-component bound of the
-    input (None = exact).  angles32: take the angles as fp32 atan2f values (the bit-level known answers of the reference).
-    Returns (q64, bound, ambiguous mask, q64 of the other wrap branch, bound to carry into the next stage)."""
-    z = np.asarray(z)
-    if angles32:
-        th = np.arctan2(z.imag.astype(np.float32), z.real.astype(np.float32)).astype(np.float64)
-    else:
-        z = z.astype(np.complex128)
-        th = np.arctan2(z.imag, z.real)
-    prev = np.concatenate([[0.0], th[:-1]])
-    raw = th - prev
-    d = raw.copy()
-    d[raw > P32] -= TWO_P
-    d[raw <= -P32] += TWO_P
-    q = d * inv_dev
-    if b is None:
-        cond = np.zeros(th.size)
-    else:
-        r = math.sqrt(2.0) * np.asarray(b, np.float64) / np.maximum(np.abs(z), 1e-300)
-        cond = np.where(r < 1.0, np.arcsin(np.minimum(r, 1.0)), np.pi)
-    A = cond + ATAN2_ULP * ulp32(np.abs(th) + cond)
-    flip = (cond > 0) & (np.pi - np.abs(th) <= A)
-    Ap = np.concatenate([[0.0], A[:-1]])
-    flipp = np.concatenate([[False], flip[:-1]])
-    E = A + Ap + U * (np.abs(th) + np.abs(prev) + A + Ap)
-    E = E + (flip.astype(np.float64) + flipp) * 2.0 * (P32 - np.pi)
-    E = E + np.where(np.abs(raw) + E >= P32, U * P32, 0.0)
-    cap = 2.0 * P32 * inv_dev * (1.0 + 2.0 * U)
-    bq = np.minimum(inv_dev * (E + U * (np.abs(d) + E)), cap)
-    amb = np.abs(np.abs(d) - P32) <= E
-    alt = (d - np.sign(d) * TWO_P) * inv_dev
-    return q, bq, amb, alt, np.where(amb, cap, bq)
-
-
-def quad_ratio(q, q64, bq, amb, alt):
-    q = np.asarray(q, np.float64)
-    err = np.abs(q - q64)
-    err = np.where(amb, np.minimum(err, np.abs(q - alt)), err)
-    return err / bq
-
-
-def deemph_coefs(tau, sr):
-    dt = np.float32(1.0 / sr)
-    a = np.float32(float(dt) / (tau + float(dt)))
-    return float(a), float(np.float32(np.float32(1.0) - a))
-
-
-def deemph_f64(x, e, a, b, y0=0.0, e0=0.0):
-    """y = a x + b y[-1] per component from state y0 (complex l + j r), with the recursion bound of the module docstring"""
-    x = np.asarray(x, np.complex128)
-    e = np.zeros(x.size) if e is None else np.asarray(e, np.float64)
-    y = lfilter([a], [1.0, -b], x, zi=np.array([b * y0], np.complex128))[0]
-    ax = np.maximum(np.abs(x.real), np.abs(x.imag))
-    yp = np.concatenate([[y0], y[:-1]])
-    ayp = np.maximum(np.abs(yp.real), np.abs(yp.imag))
-    f = a * (1 + 3 * U) * e + 3 * U * (a * ax + b * ayp)
-    beta = b * (1 + 3 * U)
-    eb = lfilter([1.0], [1.0, -beta], f, zi=np.array([beta * e0]))[0]
-    return y, eb + REF_FLOOR * float(np.abs(y).max(initial=0.0))
-
-
-def volume_f64(x, e, volume, muted):
-    g = 0.0 if muted else float(np.float32(np.float32(volume) ** np.float32(2)))
-    ax = np.maximum(np.abs(x.real), np.abs(x.imag))
-    return x * g, (e * g + U * g * (ax + e)) if g else np.zeros(x.size)
-
-
-def _ratio_c(y, y64, b):
-    """per-component error over the bound (an exact answer with a zero bound, a muted output, counts as 0)"""
-    y = np.asarray(y).astype(np.complex128)
-    err = np.maximum(np.abs(y.real - y64.real), np.abs(y.imag - y64.imag))
-    return np.where(b > 0, err / np.where(b > 0, b, 1.0), np.where(err == 0, 0.0, np.inf))
-
-
-def _chunk_index(counts):
-    """chunk of every output, from per-chunk output counts"""
-    return np.repeat(np.arange(len(counts)), counts)
-
-
-# ---------------------------------------------------------------------------------------------- the radio's VFO, in float64
-def audio_lp_taps(oracle, cfg):
-    from sdrplusplus_b200 import lib as L
-    osr = cfg.out_samplerate
-    if not cfg.low_pass:
-        return None
-    if cfg.demod == L.DEMOD_NFM:
-        return oracle.lowpass(cfg.bandwidth / 2.0, cfg.bandwidth / 2.0 * 0.1, osr)       # fm.h:123
-    return oracle.lowpass(15000.0, 4000.0, osr)                                           # broadcast_fm.h:45
-
-
-def quad_dev(cfg):
-    from sdrplusplus_b200 import lib as L
-    return cfg.bandwidth / 2.0 if cfg.demod == L.DEMOD_NFM else cfg.deviation
-
-
-def chan_taps(oracle, bw, osr):
-    return np.ones(1, np.float32) if bw == osr else oracle.lowpass(bw / 2.0, bw / 2.0 * 0.1, osr)
-
-
-def vfo_audio_f64(oracle, x, sched, fs, cfgs):
-    """one FM VFO of the front end in float64; cfgs[c] is the configuration chunk c ran with.  Returns (l + j r, bound,
-    ambiguous wraps, reach): reach is the part of the bound that comes from ill-conditioned discriminator samples (ambiguous
-    wraps and samples at the cap), carried through the same stages with |taps|."""
-    from sdrplusplus_b200 import frontend
-    c0 = cfgs[0]
-    osr = c0.out_samplerate
-    rp = frontend.resamp_plan(fs, osr)
-    pr = rp["predec_ratio"]
-    plan = [(D, oracle.decim_taps(pr, k)) for k, (D, T) in enumerate(rp["stages"])]
-    D0, h0 = plan[0]
-    PS, eps = 0, 0.0
-    for o in sorted(set(c.offset for c in cfgs)):
-        w = w_u64(o, fs)
-        ps, sg = pfb_detect([w], h0.size)
-        if ps:
-            PS, eps = max(PS, ps), max(eps, abs(pfb_eps(w, ps, sg)))
-    y, b = stage1_f64(x, sched, [c.offset for c in cfgs], h0, D0, fs, eps, PS)
-    stages = [("fir", D0)]
-    for D, h in plan[1:]:
-        y, b = fir_f64(y, b, h, D)
-        stages.append(("fir", D))
-    if rp["ntaps"]:
-        y, b = poly_f64(y, b, oracle.resamp_taps(fs, osr), rp["interp"], rp["decim"])
-        stages.append(("poly", rp["interp"], rp["decim"]))
-    # channel filter, swapped at chunk boundaries; every change passes through the identity, so each stretch of one low-pass
-    # starts from cleared history
-    ci = _chunk_index(cascade_counts(sched, stages))
-    bws = np.array([c.bandwidth for c in cfgs])[ci]
-    yc, bc = np.empty_like(y), np.empty_like(b)
-    starts = [0] + [i for i in range(1, y.size) if bws[i] != bws[i - 1]] + [y.size]
-    for s0, s1 in zip(starts[:-1], starts[1:]):
-        if s0 > 0:
-            assert bws[s0] == osr or bws[s0 - 1] == osr, "a low-pass -> low-pass change is not modelled here"
-        yc[s0:s1], bc[s0:s1] = fir_f64(y[s0:s1], b[s0:s1], chan_taps(oracle, float(bws[s0]), osr), 1)
-    inv = inv_dev_of(quad_dev(c0), osr)
-    q, bq, amb, alt, carry = quad_f64(yc, bc, inv)
-    t = np.where(amb | (bq >= 2.0 * P32 * inv), carry, 0.0)
-    h = audio_lp_taps(oracle, c0)
-    if h is not None:
-        a, ea = fir_f64(q, carry, h, 1)
-        t = fir_f64(t, None, np.abs(h), 1)[0]
-    else:
-        a, ea = q, carry
-    y, b = a + 1j * a, ea
-    if c0.af_samplerate > 0:
-        afs = c0.af_samplerate
-        ap = frontend.resamp_plan(osr, afs)
-        for k, (D, T) in enumerate(ap["stages"]):
-            h = oracle.decim_taps(ap["predec_ratio"], k)
-            y, b = fir_f64(y, b, h, D)
-            t = fir_f64(t, None, np.abs(h), D)[0]
-            stages.append(("fir", D))
-        if ap["ntaps"]:
-            h = oracle.resamp_taps(osr, afs)
-            y, b = poly_f64(y, b, h, ap["interp"], ap["decim"])
-            t = poly_f64(t, None, np.abs(h), ap["interp"], ap["decim"])[0]
-            stages.append(("poly", ap["interp"], ap["decim"]))
-        ci = _chunk_index(cascade_counts(sched, stages))
-        hp_on = np.array([c.af_high_pass for c in cfgs], bool)[ci]
-        if hp_on.any():
-            # a high-pass switched off is skipped and keeps its delay line: it filters the samples of its "on" stretches
-            hp = oracle.highpass(300.0, 100.0, afs)
-            yh, bh = fir_f64(y[hp_on], b[hp_on], hp, 1)
-            y, b, t = y.copy(), b.copy(), t.copy()
-            y[hp_on], b[hp_on], t[hp_on] = yh, bh, fir_f64(t[hp_on], None, np.abs(hp), 1)[0]
-        taus = np.array([c.af_deemph_tau for c in cfgs])[ci]
-        if (taus > 0).any():
-            assert (taus > 0).all(), "de-emphasis switched off is not modelled here"
-            yo, bo, to = np.empty_like(y), np.empty_like(b), np.empty_like(t)
-            y0, e0, t0 = 0.0, 0.0, 0.0
-            cut = [0] + [i for i in range(1, y.size) if taus[i] != taus[i - 1]] + [y.size]
-            for s0, s1 in zip(cut[:-1], cut[1:]):
-                aa, bb = deemph_coefs(float(taus[s0]), afs)
-                yo[s0:s1], bo[s0:s1] = deemph_f64(y[s0:s1], b[s0:s1], aa, bb, y0, e0)
-                to[s0:s1] = lfilter([aa], [1.0, -bb], t[s0:s1], zi=np.array([bb * t0]))[0]
-                if s1 > s0:
-                    y0, e0, t0 = yo[s1 - 1], bo[s1 - 1], to[s1 - 1]
-            y, b, t = yo, bo, to
-    if any(c.af_volume_on for c in cfgs):
-        ci = _chunk_index(cascade_counts(sched, stages))
-        yv, bv = np.empty_like(y), np.empty_like(b)
-        for k, c in enumerate(cfgs):
-            sel = ci == k
-            if c.af_volume_on:
-                yv[sel], bv[sel] = volume_f64(y[sel], b[sel], c.af_volume, c.af_muted)
-                t = t.copy()
-                t[sel] *= 0.0 if c.af_muted else float(np.float32(np.float32(c.af_volume) ** np.float32(2)))
-            else:
-                yv[sel], bv[sel] = y[sel], b[sel]
-        y, b = yv, bv
-    return y, b, int(amb.sum()), t
-
-
-def vfo_counts(oracle, fs, cfg, sched):
-    from sdrplusplus_b200 import frontend
-    rp = frontend.resamp_plan(fs, cfg.out_samplerate)
-    st = [("fir", D) for D, T in rp["stages"]] + ([("poly", rp["interp"], rp["decim"])] if rp["ntaps"] else [])
-    if cfg.af_samplerate > 0:
-        ap = frontend.resamp_plan(cfg.out_samplerate, cfg.af_samplerate)
-        st += [("fir", D) for D, T in ap["stages"]] + ([("poly", ap["interp"], ap["decim"])] if ap["ntaps"] else [])
-    return cascade_counts(sched, st)
 
 
 # ---------------------------------------------------------------------------------------------- routing mirror
@@ -785,28 +567,6 @@ def _audio_gate(parts, y64, b, reach, restarts=()):
     g = _gate_clean(y[:, 0].astype(np.float64), y64.real, clean, [p.shape[0] for p in parts], restarts)
     return dict(g, max_err_over_bound=float(r[k]) if r.size else 0.0, worst_output=k)
 
-
-def _gate_clean(y, yo, clean, counts, restarts=()):
-    """f64_ref._gate_vfo's fitted gain and edge-against-interior ratio over the outputs in `clean`; the stream's first EDGE
-    outputs (the start transient, where the partly filled windows give the discriminator small |z|), and the first EDGE
-    outputs of each chunk in `restarts` (a filter restarted from cleared history), count as neither edge nor interior"""
-    edge = np.zeros(y.size, bool)
-    for bnd in np.cumsum(counts[:-1]):
-        edge[max(0, bnd - EDGE): bnd + EDGE] = True
-    clean = clean.copy()
-    clean[:EDGE] = False
-    for k in restarts:
-        at = int(sum(counts[:k]))
-        clean[at: at + EDGE] = False
-    assert (edge & clean).any() and (~edge & clean).sum() >= 1000
-    yc, oc = y[clean], yo[clean]
-    g = float(np.dot(oc, yc) / np.dot(oc, oc))
-    e = np.abs(y - yo) / math.sqrt(float(np.mean(oc ** 2)))
-    p999 = float(np.percentile(e[~edge & clean], 99.9))
-    emax = float(e[edge & clean].max())
-    ratio = emax / p999 if p999 > 0 else (0.0 if emax == 0 else np.inf)
-    return {"rel_rms": float(np.linalg.norm(yc - oc) / np.linalg.norm(oc)), "gain": g, "abs_g_minus_1": abs(g - 1.0),
-            "edge_over_p999": ratio, "outputs": int(y.size), "gated_outputs": int(clean.sum())}
 
 
 def _check(res, name):
