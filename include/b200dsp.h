@@ -285,18 +285,20 @@ int b200_fe_submit(b200_fe* fe, const void* iq, int count, int in_fmt, int in_me
 int b200_fe_wait(b200_fe* fe);
 /* number of kernels this handle has launched so far (bench.py's gpu_launches) */
 long long b200_fe_launch_count(b200_fe* fe);
-/* counters by name: "launches", "chunks", "s1_tma_launches" (stage-1 launches of this process that ran the TMA-fed
+/* counters by name: "launches", "chunks", "s1_tma_launches" (stage-1 launches of this handle that ran the TMA-fed
  * filter-bank kernel), "s1_f2_jobs" (VFO-chunks of this handle whose (4, 27) decimating FIR ran inside that kernel), "graphs" / "graph_hits" / "graph_misses" (launch lists captured / replayed / launched plainly),
  * "host_ns_plan" / "host_ns_fft" / "host_ns_run" / "host_ns_join" / "host_ns_stage1" / "host_ns_tail" (host time spent inside
  * b200_fe_submit since creation, by section, in ns), "fused_chains" (VFOs whose stages behind stage 1 are planned into one
  * k_tail_fused launch per chunk); -1 for an unknown key */
 long long b200_fe_stat(b200_fe* fe, const char* key);
-/* Tuning / A-B switches (defaults are the fast paths; every variant is held to the same parity tests):
+/* Tuning / A-B switches (defaults are the fast paths; every variant is held to the same parity tests).  Every option applies
+ * to the front end it is set on and to no other handle; stand-alone handles (b200_block, b200_fft, b200_chan) use the defaults.
  *  "s1"      stage-1 kernel: 8 (default) filter-bank form fed by the TMA engine (cf32 chunks, VFO offsets on a common
  *            frequency grid, first decimation 32 or 64); 7 the same form on cp.async tiles; 6 per-VFO complex taps on
  *            cp.async tiles, one tile buffer per CTA, three 4-warp CTAs per SM; 5 the same double-buffered, one CTA per SM;
  *            0 one thread per output.  Each falls through to the next when a plan does not fit it.
- *            "s1_stages" ring depth of the TMA kernel (2 default, 3); "pair" 1 = VFOs at +f / -f share their stage-1 sums
+ *            "s1_stages" ring depth of the TMA kernel (2 default, 3); "s1_mt" tile of the per-VFO cp.async kernel in outputs,
+ *            rounded down to a multiple of 128 (0 = automatic); "pair" 1 = VFOs at +f / -f share their stage-1 sums
  *  "tails"   2 (default): every stage behind stage 1 that has a register-window kernel runs in it (k_dfir_reg, k_poly_reg,
  *            k_fir_reg, k_firr_reg; "ft_prereg" caps how many leading decimating FIRs may, "ft_regall" 0 keeps the others in
  *            the fused launch k_tail_fused, tuned by "ft_threads", "ft_obmax", "ft_ob", "ft_smem_kb", "ft_direct");
@@ -317,11 +319,11 @@ long long b200_fe_stat(b200_fe* fe, const char* key);
  *  "s1_ctas" persistent CTAs of the TMA stage 1 (0 = one per SM)
  *  "pdl"     programmatic dependent launch for the chain kernels behind stage 1 (a successor is scheduled and loads its tables
  *            under its predecessor, and touches the stage buffers behind griddepcontrol.wait): 2 (default) launches of at most
- *            two CTAs per SM -- the small grids of chunks up to about 1e6 samples --, 1 every launch, 0 never.  Process-wide;
- *            also the environment variable B200_PDL
+ *            two CTAs per SM -- the small grids of chunks up to about 1e6 samples --, 1 every launch, 0 never.  The environment
+ *            variable B200_PDL, read once per process, sets the default
  *  "s1_diag" measurement only (outputs are garbage): 1 = the TMA stage 1 loads its tiles but does not filter them, 2 = it
  *            filters whatever its tile buffers hold and loads nothing -- what the ring alone and the consumer warps alone
- *            sustain (tools/s1_bounds.py); reset to 0 by every b200_fe_create
+ *            sustain (tools/s1_bounds.py)
  *  "time_s1" 1 = bracket the launch groups of every chunk with CUDA events (b200_fe_s1_stats / b200_fe_group_stats) */
 int b200_fe_set_option(b200_fe* fe, const char* key, int value);
 /* device time spent in the stage-1 (translate + first decimation) launches since the last call, and their count;

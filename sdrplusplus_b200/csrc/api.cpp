@@ -283,7 +283,8 @@ static size_t iq_tap_bytes(int type) {
 struct b200_fe {
     double fs = 0;
     int max_chunk = 0;
-    Scheduler sch;
+    KernelOpts opts;             // the kernel choices of this front end (b200_fe_set_option); sch and sch_pre launch with them
+    Scheduler sch{opts};
     cudaStream_t own_stream = nullptr, copy_stream = nullptr, fft_stream = nullptr, tail_stream = nullptr, join_stream = nullptr;
     cudaEvent_t ev_tail_done[FE_SLOTS] = {};
     cudaEvent_t ev_fft_go = nullptr, ev_fft_done = nullptr, ev_lines_free = nullptr;
@@ -319,7 +320,7 @@ struct b200_fe {
     double fs_eff = 0;
     bool dc_block = false, invert_iq = false;
     Chain pre;                   // the decimator (typed cf32 chain), built when decim > 1
-    Scheduler sch_pre;
+    Scheduler sch_pre{opts};
     DevBuf pp[FE_SLOTS];         // chunk after DC blocker / conjugate (one per chunk in flight)
     DevBuf dc_state, dc_segA, dc_segB;
     int max_eff = 0;             // largest chunk behind the decimator
@@ -375,8 +376,6 @@ extern "C" b200_fe* b200_fe_create(double samplerate, int max_chunk) {
     }
     fe->sch.stream = fe->own_stream;
     fe->sch.fuse.on = true;
-    kernels_set_xd_tma_stages(2);          // process-wide tuning knobs start from their defaults with every new front end
-    kernels_set_xd_tma_diag(0);
     {
         int dev = 0, sms = 0;
         if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && sms > 0) {
@@ -774,11 +773,10 @@ extern "C" int b200_fe_fft_max_lines(b200_fe* fe, int count) {
     return (int)(count / ((long long)fe->fft.nz + fe->skip)) + 2;
 }
 extern "C" long long b200_fe_launch_count(b200_fe* fe) { return fe ? fe->sch.launches : 0; }
-extern int g_xd_tma_launches;
 extern "C" long long b200_fe_stat(b200_fe* fe, const char* key) {
     if (!fe || !key) { return -1; }
     if (!strcmp(key, "launches")) { return fe->sch.launches; }
-    if (!strcmp(key, "s1_tma_launches")) { return g_xd_tma_launches; }      // process-wide: stage-1 launches that took the TMA kernel
+    if (!strcmp(key, "s1_tma_launches")) { return fe->sch.s1_tma_launches; }
     if (!strcmp(key, "s1_f2_jobs")) { return fe->sch.s1_f2_jobs; }
     if (!strcmp(key, "chunks")) { return (long long)fe->nsub; }
     // host time spent inside b200_fe_submit since creation, by section (ns)
@@ -798,6 +796,11 @@ extern "C" long long b200_fe_stat(b200_fe* fe, const char* key) {
     }
     return -1;
 }
+// the captured graphs of both schedulers hold launches made with the old kernel choices
+static void fe_drop_graphs(b200_fe* fe) {
+    fe->sch.drop_graphs();
+    fe->sch_pre.drop_graphs();
+}
 extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {
     if (!fe || !key) { set_error("null argument"); return B200_EINVAL; }
     if (!strcmp(key, "s1")) { fe->sch.s1_variant = value; return 0; }
@@ -808,15 +811,14 @@ extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {
         return 0;
     }
     if (!strcmp(key, "pair")) { fe->sch.pair_conjugates = value != 0; return 0; }
-    if (!strcmp(key, "s1_mt")) { kernels_set_xd_tile(value); return 0; }
-    if (!strcmp(key, "s1_cps")) { kernels_set_xd_cps(value); return 0; }
-    if (!strcmp(key, "s1_stages")) { kernels_set_xd_tma_stages(value); return 0; }
-    if (!strcmp(key, "s1_diag")) { kernels_set_xd_tma_diag(value); return 0; }                   // measurement only: outputs are garbage
-    if (!strcmp(key, "s1_ctas")) { kernels_set_xd_tma_ctas(value); return 0; }
+    if (!strcmp(key, "s1_mt")) { fe->opts.s1_mt = value; return 0; }
+    if (!strcmp(key, "s1_stages")) { fe->opts.s1_stages = value == 3 ? 3 : 2; return 0; }
+    if (!strcmp(key, "s1_diag")) { fe->opts.s1_diag = value & 3; return 0; }                     // measurement only: outputs are garbage
+    if (!strcmp(key, "s1_ctas")) { fe->opts.s1_ctas = value; return 0; }
     if (!strcmp(key, "tails") || !strncmp(key, "ft_", 3)) {
         // 0: one thread per output; 1: shared-memory tiled kernels, one launch per stage; 2: one fused launch per <= 16 VFOs
         if (b200_fe_vfo_count(fe) > 0) { set_error("'%s' must be chosen before VFOs are added", key); return B200_ESTATE; }
-        if (!strcmp(key, "tails")) { kernels_set_tail_variant(value >= 1 ? 1 : 0); fe->sch.fuse.on = value >= 2; return 0; }
+        if (!strcmp(key, "tails")) { fe->opts.tail_variant = value >= 1 ? 1 : 0; fe->sch.fuse.on = value >= 2; fe_drop_graphs(fe); return 0; }
         if (!strcmp(key, "ft_ob")) { fe->sch.fuse.ob_force = value; return 0; }
         if (!strcmp(key, "ft_obmax")) { fe->sch.fuse.ob_max = value; return 0; }
         if (!strcmp(key, "ft_smem_kb")) { fe->sch.fuse.smem_limit = value * 1024; return 0; }
@@ -825,8 +827,8 @@ extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {
         if (!strcmp(key, "ft_prereg")) { fe->sch.fuse.pre_reg = value; return 0; }
         if (!strcmp(key, "ft_regall")) { fe->sch.fuse.reg_all = value != 0; return 0; }
     }
-    if (!strcmp(key, "fft")) { kernels_set_fft_variant(value); return 0; }
-    if (!strcmp(key, "fft_cta")) { kernels_set_fft_cta(value); return 0; }
+    if (!strcmp(key, "fft")) { fe->opts.fft_variant = value; return 0; }
+    if (!strcmp(key, "fft_cta")) { fe->opts.fft_cta = value == 4 ? 4 : 8; return 0; }
     if (!strcmp(key, "host_direct")) { fe->host_direct = value; return 0; }
     if (!strcmp(key, "inflight")) {
         if (value < 1 || value > FE_SLOTS) { set_error("inflight: 1 ... %d", FE_SLOTS); return B200_EINVAL; }
@@ -841,7 +843,7 @@ extern "C" int b200_fe_set_option(b200_fe* fe, const char* key, int value) {
     }
     if (!strcmp(key, "graph")) { fe->sch.graph_tails = value; if (value == 0) { fe->sch.drop_graphs(); } return 0; }
     if (!strcmp(key, "graph_max_count")) { fe->sch.graph_max_count = value; return 0; }
-    if (!strcmp(key, "pdl")) { kernels_set_pdl(value); fe->sch.drop_graphs(); return 0; }      // process-wide, like the kernel variants
+    if (!strcmp(key, "pdl")) { fe->opts.pdl = (value >= 0 && value <= 2) ? value : PDL_DEFAULT; fe_drop_graphs(fe); return 0; }
     if (!strcmp(key, "time_s1")) { fe->sch.time_s1 = value != 0; for (auto& t : fe->sch.timers) { t.used = 0; } return 0; }
     set_error("unknown option %s", key);
     return B200_EINVAL;
@@ -1303,7 +1305,8 @@ static int fe_fft_chunk(b200_fe* fe, FeChunk& c) {
             if ((rc = fork())) { return rc; }
             int nl = 0;
             const FftFrames fr{ fe->frame.p, nullptr, 0, 0, 1 };
-            cudaError_t e = launch_fft_frames(fe->fft.plan, fr, FMT_CF32, fe->fft.work.as<float2>(), lines_base, nullptr, s, &nl, fe->fft_v != 0);
+            cudaError_t e = launch_fft_frames(fe->fft.plan, fr, FMT_CF32, fe->fft.work.as<float2>(), lines_base, nullptr, fe->opts, s, &nl,
+                                              fe->fft_v != 0);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_fft_frames"); }
             fe->sch.launches += nl;
             c.nlines++;
@@ -1326,7 +1329,7 @@ static int fe_fft_chunk(b200_fe* fe, FeChunk& c) {
         const FftFrames fr{ (const char*)c.ein + (size_t)(fe->fstart + split - pos) * bps, frame, (long long)interval, (int)split, nb };
         int nl = 0;
         cudaError_t e = launch_fft_frames(fe->fft.plan, fr, c.efmt, fe->fft.work.as<float2>(), lines_base + (size_t)c.nlines * fe->fft.size,
-                                          nullptr, s, &nl, fe->fft_v != 0);
+                                          nullptr, fe->opts, s, &nl, fe->fft_v != 0);
         if (e != cudaSuccess) { return cuda_fail(e, "launch_fft_frames"); }
         fe->sch.launches += nl;
         c.nlines += nb;
@@ -1566,7 +1569,8 @@ extern "C" int b200_fft_zoom_hold(const float* line, int fft_size, int offset, i
 // ------------------------------------------------------------------ stand-alone blocks
 struct b200_block {
     Chain chain;
-    Scheduler sch;
+    KernelOpts opts;      // the defaults: a block has no kernel options
+    Scheduler sch{opts};
     cudaStream_t stream = nullptr;
     DevBuf in_dev;        // raw chains: the chunk as uploaded
     int in_es = 2;
@@ -1909,7 +1913,7 @@ static int fft_run(b200_fft* f, const float* iq, float* out_db, float* out_c) {
     if (!f || !iq) { set_error("null argument"); return B200_EINVAL; }
     B200_CK(cudaMemcpy(f->in.p, iq, (size_t)f->core.nz * sizeof(float2), cudaMemcpyHostToDevice));
     cudaError_t e = launch_fft_frame(f->core.plan, f->in.p, FMT_CF32, f->core.work.as<float2>(), f->db.as<float>(),
-                                     f->raw.as<float2>(), 0, nullptr);
+                                     f->raw.as<float2>(), KernelOpts(), 0, nullptr);
     if (e != cudaSuccess) { return cuda_fail(e, "launch_fft_frame"); }
     if (out_db) { B200_CK(cudaMemcpy(out_db, f->db.p, (size_t)f->core.size * sizeof(float), cudaMemcpyDeviceToHost)); }
     if (out_c) { B200_CK(cudaMemcpy(out_c, f->raw.p, (size_t)f->core.size * sizeof(float2), cudaMemcpyDeviceToHost)); }
@@ -2294,7 +2298,7 @@ extern "C" int b200_chan_process(b200_chan* c, const void* iq, int count, int in
         CarryJob& j = cp.job[0];
         j.dst = c->inbuf.as<float>(); j.a = c->inbuf.as<float>(); j.b = data;
         j.h = (int)hist; j.la = (int)hist; j.lb = count; j.esize = 2; j.bfmt = -1; j.scale = 0.0f;
-        e = launch_carry(cp, s);
+        e = launch_carry(cp, KernelOpts(), s);
         if (e != cudaSuccess) { return cuda_fail(e, "launch_carry"); }
         nl++;
     }

@@ -92,9 +92,9 @@ __global__ void __launch_bounds__(DFR_THREADS) k_dfir_reg(const __grid_constant_
 }
 
 template <int D, int T, int R>
-static cudaError_t launch_dfir_reg_t(const DfrParams& p, cudaStream_t s) {
+static cudaError_t launch_dfir_reg_t(const DfrParams& p, const KernelOpts& o, cudaStream_t s) {
     dim3 grid((unsigned)((p.max_out + DFR_THREADS * R - 1) / (DFR_THREADS * R)), (unsigned)p.njobs);
-    return launch_chain(k_dfir_reg<D, T, R>, grid, dim3(DFR_THREADS), DfrGeom<D, T, R>::SMEM, s, p);
+    return launch_chain(k_dfir_reg<D, T, R>, grid, dim3(DFR_THREADS), DfrGeom<D, T, R>::SMEM, o, s, p);
 }
 // true when (D, T) is one of the plan stages the kernel is built for
 bool dfir_reg_supported(int D, int T) {
@@ -102,13 +102,13 @@ bool dfir_reg_supported(int D, int T) {
 }
 // every job: same D and T (p.taps holds the common taps).  The reads run up to one sample past the last one an output
 // needs (16-byte granularity): stage buffers carry 8 spare samples (Stage::alloc_in).
-cudaError_t launch_dfir_reg(const DfrParams& p, int D, int T, cudaStream_t s) {
+cudaError_t launch_dfir_reg(const DfrParams& p, int D, int T, const KernelOpts& o, cudaStream_t s) {
     if (p.njobs <= 0 || p.max_out <= 0) { return cudaSuccess; }
-    if (D == 4 && T == 27) { return launch_dfir_reg_t<4, 27, 8>(p, s); }
-    if (D == 2 && T == 69) { return launch_dfir_reg_t<2, 69, 4>(p, s); }
-    if (D == 2 && T == 12) { return launch_dfir_reg_t<2, 12, 8>(p, s); }
-    if (D == 8 && T == 54) { return launch_dfir_reg_t<8, 54, 4>(p, s); }
-    if (D == 8 && T == 44) { return launch_dfir_reg_t<8, 44, 4>(p, s); }
-    if (D == 8 && T == 36) { return launch_dfir_reg_t<8, 36, 4>(p, s); }
+    if (D == 4 && T == 27) { return launch_dfir_reg_t<4, 27, 8>(p, o, s); }
+    if (D == 2 && T == 69) { return launch_dfir_reg_t<2, 69, 4>(p, o, s); }
+    if (D == 2 && T == 12) { return launch_dfir_reg_t<2, 12, 8>(p, o, s); }
+    if (D == 8 && T == 54) { return launch_dfir_reg_t<8, 54, 4>(p, o, s); }
+    if (D == 8 && T == 44) { return launch_dfir_reg_t<8, 44, 4>(p, o, s); }
+    if (D == 8 && T == 36) { return launch_dfir_reg_t<8, 36, 4>(p, o, s); }
     return cudaErrorInvalidValue;
 }

@@ -979,32 +979,37 @@ unsigned long long LaunchRec::hash() const {
     for (size_t i = n8 * 8; i < bytes.size(); i++) { mix(b[i]); }
     return h;
 }
-int LaunchRec::replay(cudaStream_t s, long long* nlaunch) const {
+int LaunchRec::replay(const KernelOpts& o, cudaStream_t s, long long* nlaunch) const {
     for (const Item& it : items) {
         int nl = 0;
-        cudaError_t e = it.fn(bytes.data() + it.off, it, s, &nl);
+        cudaError_t e = it.fn(bytes.data() + it.off, it, o, s, &nl);
         if (e != cudaSuccess) { return cuda_fail(e, "kernel launch (tail list)"); }
         if (nlaunch) { *nlaunch += nl; }
     }
     return 0;
 }
 
-// the launchers of the list: one per typed launch function
+// the launchers of the list: one per typed launch function, with or without kernel choices
+template <class P, cudaError_t (*L)(const P&, const KernelOpts&, cudaStream_t)>
+static cudaError_t launch_of(const void* p, const LaunchRec::Item&, const KernelOpts& o, cudaStream_t s, int* nl) {
+    *nl = 1;
+    return L(*(const P*)p, o, s);
+}
 template <class P, cudaError_t (*L)(const P&, cudaStream_t)>
-static cudaError_t launch_of(const void* p, const LaunchRec::Item&, cudaStream_t s, int* nl) {
+static cudaError_t launch_of(const void* p, const LaunchRec::Item&, const KernelOpts&, cudaStream_t s, int* nl) {
     *nl = 1;
     return L(*(const P*)p, s);
 }
 template <class P, cudaError_t (*L)(const P&, cudaStream_t, int*)>        // launch_stereo, launch_squelch: more than one kernel
-static cudaError_t launch_of_n(const void* p, const LaunchRec::Item&, cudaStream_t s, int* nl) {
+static cudaError_t launch_of_n(const void* p, const LaunchRec::Item&, const KernelOpts&, cudaStream_t s, int* nl) {
     return L(*(const P*)p, s, nl);
 }
-static cudaError_t launch_of_dfr(const void* q, const LaunchRec::Item&, cudaStream_t s, int* nl) {
+static cudaError_t launch_of_dfr(const void* q, const LaunchRec::Item&, const KernelOpts& o, cudaStream_t s, int* nl) {
     const DfrParams& p = *(const DfrParams*)q;                              // every job of a batch: the same D and T
     *nl = 1;
-    return launch_dfir_reg(p, p.job[0].decim, p.job[0].ntaps, s);
+    return launch_dfir_reg(p, p.job[0].decim, p.job[0].ntaps, o, s);
 }
-static cudaError_t launch_of_ft(const void* q, const LaunchRec::Item& it, cudaStream_t s, int* nl) {
+static cudaError_t launch_of_ft(const void* q, const LaunchRec::Item& it, const KernelOpts&, cudaStream_t s, int* nl) {
     const FtParams& p = *(const FtParams*)q;
     int max_slabs = 0;
     for (int i = 0; i < p.njobs; i++) { max_slabs = std::max(max_slabs, p.job[i].slabs); }
@@ -1080,7 +1085,7 @@ int Scheduler::apply_deferred(std::vector<Chain*>& chains) {
 // the recorded launch list of this chunk: first sight -> plain launches; second sight -> capture into a graph; then replay
 int Scheduler::launch_recorded(cudaStream_t ts, bool may_graph) {
     if (rec.items.empty()) { return 0; }
-    if (!may_graph) { return rec.replay(ts, &launches); }
+    if (!may_graph) { return rec.replay(opts, ts, &launches); }
     const unsigned long long h = rec.hash();
     auto it = graphs.find(h);
     if (it != graphs.end() && it->second.key.size() == rec.bytes.size() && memcmp(it->second.key.data(), rec.bytes.data(), rec.bytes.size()) == 0) {
@@ -1094,7 +1099,7 @@ int Scheduler::launch_recorded(cudaStream_t ts, bool may_graph) {
         // second sight: capture
         if (cudaStreamBeginCapture(ts, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
             long long nl = 0;
-            int rc = rec.replay(ts, &nl);
+            int rc = rec.replay(opts, ts, &nl);
             cudaGraph_t graph = nullptr;
             cudaError_t e = cudaStreamEndCapture(ts, &graph);
             cudaGraphExec_t exec = nullptr;
@@ -1111,7 +1116,7 @@ int Scheduler::launch_recorded(cudaStream_t ts, bool may_graph) {
             cudaGetLastError();
             graph_tails = 0;                       // capture is not possible here: plain launches from now on
         }
-        return rec.replay(ts, &launches);
+        return rec.replay(opts, ts, &launches);
     }
     if (graphs.size() >= 256) { drop_graphs(); }
     GraphEntry& g = graphs[h];
@@ -1119,7 +1124,7 @@ int Scheduler::launch_recorded(cudaStream_t ts, bool may_graph) {
     g.key = rec.bytes;
     g.launches = 0;
     graph_misses++;
-    return rec.replay(ts, &launches);
+    return rec.replay(opts, ts, &launches);
 }
 
 static inline long long host_now_ns() {
@@ -1293,10 +1298,11 @@ int Scheduler::stage1(std::vector<Chain*>& chains, const void* raw, int fmt, int
                 if (g[b + v]->gpad_len < (p.D - 1) + (p.QP + 8) * p.D) { variant = 0; }
             }
             int nl = 0;
-            bool f2 = false;
+            bool tma = false, f2 = false;
             cudaEvent_t t1 = timer_begin(0, stream);
-            cudaError_t e = launch_xlate_decim(p, fmt, variant, stream, &nl, &f2);
+            cudaError_t e = launch_xlate_decim(p, fmt, variant, opts, stream, &nl, &tma, &f2);
             if (e != cudaSuccess) { return cuda_fail(e, "launch_xlate_decim"); }
+            if (tma) { s1_tma_launches++; }
             // ÷4-epilogue bookkeeping: which (4, 27) stages stage 1 computed this chunk
             for (int v = 0; v < p.njobs; v++) {
                 Chain* c = chain_of[g[b + v]];
@@ -1320,7 +1326,7 @@ int Scheduler::carry_raw_hist(const void* raw, int fmt, int count) {
     CarryJob& j = rc1.job[0];
     j.dst = raw_hist.as<float>(); j.a = raw_hist.as<float>(); j.b = raw;
     j.h = RAW_HIST; j.la = RAW_HIST; j.lb = count; j.esize = 2; j.bfmt = fmt; j.scale = in_scale;
-    cudaError_t e = launch_carry(rc1, stream);
+    cudaError_t e = launch_carry(rc1, opts, stream);
     if (e != cudaSuccess) { return cuda_fail(e, "launch_carry"); }
     launches++;
     return 0;

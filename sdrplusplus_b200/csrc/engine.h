@@ -298,19 +298,22 @@ void clear_stage_state(Stage& s);
 struct LaunchRec {
     struct Item;
     // a typed launch function behind a type-erased pointer (engine.cpp: launch_of); *nl = the kernels it enqueued
-    typedef cudaError_t (*Launch)(const void* params, const Item& it, cudaStream_t s, int* nl);
+    typedef cudaError_t (*Launch)(const void* params, const Item& it, const KernelOpts& o, cudaStream_t s, int* nl);
     struct Item { Launch fn; size_t off, size; int a; size_t b; };    // a, b: launch arguments outside the parameter block
     std::vector<Item> items;
     std::vector<unsigned char> bytes;
     void clear() { items.clear(); bytes.clear(); }
     void add(Launch fn, const void* p, size_t size, int a = 0, size_t b = 0);
     unsigned long long hash() const;
-    int replay(cudaStream_t s, long long* nlaunch) const;     // the real launches, in order
+    int replay(const KernelOpts& o, cudaStream_t s, long long* nlaunch) const;     // the real launches, in order
 };
 
 // Runs a set of chains over one chunk: stage-1 launches grouped by decimation, then level by level one
 // launch per stage kind, then the history carry.
 struct Scheduler {
+    // the kernel choices of the handle that owns this scheduler (a front end's two schedulers share its one instance)
+    const KernelOpts& opts;
+    explicit Scheduler(const KernelOpts& o) : opts(o) {}
     cudaStream_t stream = nullptr;
     // overlapped mode: stage 1 (+ raw history carry) runs on `stream`, every later stage on `tail_stream`, so the
     // tails of chunk k overlap stage 1 of chunk k+1.  The stage fed by stage 1 is double-buffered (Stage::dbl).
@@ -321,6 +324,7 @@ struct Scheduler {
     int enable_overlap(cudaStream_t tail);
     long long launches = 0;
     long long s1_f2_jobs = 0;    // VFO-chunks whose (4, 27) stage stage 1 computed (k_xd_tma's ÷4 epilogue; b200_fe_stat "s1_f2_jobs")
+    long long s1_tma_launches = 0;   // stage-1 launches that ran k_xd_tma (b200_fe_stat "s1_tma_launches")
     // CUDA graphs of the launch list (LaunchRec): -1 = for chunks up to graph_max_count samples, 0 = never (plain replay), 1 = always
     int graph_tails = -1;
     int graph_max_count = 1 << 30;

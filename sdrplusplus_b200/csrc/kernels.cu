@@ -89,13 +89,14 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
 // wait, never with the non-coherent path: the CTA was resident before those lines were written.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-#define PDL_DEFAULT 2
-static int g_pdl = -1;                               // 0 off, 1 always, 2 small grids only; -1: read B200_PDL once (else PDL_DEFAULT)
-int kernels_pdl() {
-    if (g_pdl < 0) { const char* e = getenv("B200_PDL"); g_pdl = e ? atoi(e) : PDL_DEFAULT; if (g_pdl < 0 || g_pdl > 2) { g_pdl = PDL_DEFAULT; } }
-    return g_pdl;
+int kernels_pdl_default() {
+    static const int mode = [] {
+        const char* e = getenv("B200_PDL");
+        const int m = e ? atoi(e) : PDL_DEFAULT;
+        return (m < 0 || m > 2) ? PDL_DEFAULT : m;
+    }();
+    return mode;
 }
-void kernels_set_pdl(int mode) { g_pdl = (mode >= 0 && mode <= 2) ? mode : PDL_DEFAULT; }
 static int num_sms();
 // <<<>>> with the programmatic-serialization attribute (captured into graphs as programmatic edges).  Mode 2, the default,
 // gives it to launches of at most two CTAs per SM: with the small grids of the reference's own chunk sizes (<= 1e6 samples)
@@ -103,13 +104,12 @@ static int num_sms();
 // 16 Mi-sample chunk the successor's waiting CTAs take shared memory and registers from the spectrum branch on the other
 // stream, which is what bounds the step there.
 template <class P>
-static cudaError_t launch_chain(void (*k)(const P), dim3 grid, dim3 block, size_t smem, cudaStream_t s, const P& p) {
+static cudaError_t launch_chain(void (*k)(const P), dim3 grid, dim3 block, size_t smem, const KernelOpts& o, cudaStream_t s, const P& p) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
     cudaLaunchAttribute at[1];
-    const int mode = kernels_pdl();
-    if (mode == 1 || (mode == 2 && (long long)grid.x * grid.y * grid.z <= 2LL * num_sms())) {
+    if (o.pdl == 1 || (o.pdl == 2 && (long long)grid.x * grid.y * grid.z <= 2LL * num_sms())) {
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
@@ -699,12 +699,6 @@ __global__ void __launch_bounds__(256) k_zoom_hold(const float* __restrict__ lin
 // launch wrappers
 // ------------------------------------------------------------------------------------------------
 static int g_smem_optin = -1;
-static int g_fft_variant = 1;     // 1: register-resident four-step passes where they apply; 0: shared-memory radix-8 passes
-void kernels_set_fft_variant(int v) { g_fft_variant = v; }
-int g_xd_tma_ctas = 0;            // persistent CTAs of the TMA stage 1 (0 = one per SM)
-void kernels_set_xd_tma_ctas(int v) { g_xd_tma_ctas = v; }
-static int g_fft_cta = 8;         // column / row transforms per CTA of the register-resident passes: 8 or 4
-void kernels_set_fft_cta(int v) { g_fft_cta = (v == 4) ? 4 : 8; }
 int kernels_max_smem_optin() {
     if (g_smem_optin < 0) {
         int dev = 0, v = 0;
@@ -735,10 +729,6 @@ static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b)
 #include "tails_reg.cuh"
 
 
-int g_xd_cps = 0;                 // cap on stage-1 CTAs per SM (0 = as many as fit): leaves room for the other streams
-void kernels_set_xd_cps(int v) { g_xd_cps = v; }
-int g_xd_mt_override = 0;
-void kernels_set_xd_tile(int mt) { g_xd_mt_override = mt; }
 static int g_num_sms = -1;
 static int num_sms() {
     if (g_num_sms < 0) {
@@ -768,7 +758,7 @@ static cudaError_t launch_xd_pipe_t(const XdParams& p, const XpGeom& g, size_t s
 
 // returns true when the pipelined kernel was launched
 template <int FMT>
-static bool try_xd_pipe(const XdParams& p, cudaStream_t s, cudaError_t* err, int nwarps, bool single = false) {
+static bool try_xd_pipe(const XdParams& p, const KernelOpts& o, cudaStream_t s, cudaError_t* err, int nwarps, bool single = false) {
     const int D = p.D;
     if (D < 2 || (D & (D - 1))) { return false; }
     int logD = 0;
@@ -810,7 +800,7 @@ static bool try_xd_pipe(const XdParams& p, cudaStream_t s, cudaError_t* err, int
     const int limit = kernels_max_smem_optin();
     // tile: about 8K raw samples (4K for the 4-warp configuration), a multiple of 128 outputs
     int MT = ((nwarps == 4 ? 4096 : 8192) / D) / 128 * 128;
-    if (g_xd_mt_override > 0) { MT = g_xd_mt_override / 128 * 128; }
+    if (o.s1_mt > 0) { MT = o.s1_mt / 128 * 128; }
     if (MT < 128) { MT = 128; }
     if (MT > 1024) { MT = 1024; }
     XpGeom g;
@@ -858,7 +848,6 @@ static cudaError_t launch_xd_pfb_t(const XdParams& p, const XpGeom& g, int fmt, 
     if (e != cudaSuccess) { return e; }
     int per_sm = (int)((size_t)233472 / (smem + 1024));
     if (per_sm > 3) { per_sm = 3; }
-    if (g_xd_cps > 0 && per_sm > g_xd_cps) { per_sm = g_xd_cps; }
     if (per_sm < 1) { per_sm = 1; }
     int grid = num_sms() * per_sm;
     if (grid > g.ntiles) { grid = g.ntiles; }
@@ -918,11 +907,6 @@ static PFN_tmap_encode tmap_encode_fn() {
     }
     return fn;
 }
-int g_xd_tma_launches = 0;        // diagnostic: how many stage-1 launches took the TMA path
-int g_xd_tma_stages = 2;          // ring depth of the TMA stage 1: 2 leaves a third of the SM's shared memory to the kernels of the other streams
-void kernels_set_xd_tma_stages(int n) { g_xd_tma_stages = (n == 3) ? 3 : 2; }
-static int g_xd_tma_diag = 0;     // XtGeom::diag (measurement only)
-void kernels_set_xd_tma_diag(int v) { g_xd_tma_diag = v & 3; }
 template <int LOGD, int QC, int PS, int MT, int NST>
 static cudaError_t launch_xd_tma_n(const XdParams& p, const XtGeom& g, const CUtensorMap& tm, int grid, cudaStream_t s) {
     using Lay = XtLay<LOGD, QC, MT>;
@@ -942,14 +926,13 @@ static cudaError_t launch_xd_tma_n(const XdParams& p, const XtGeom& g, const CUt
         attr_set = true;
     }
     k_xd_tma<LOGD, QC, PS, MT, NST><<<grid, (Lay::NW + 1) * 32, smem, s>>>(p, g, tm);
-    g_xd_tma_launches++;
     return cudaGetLastError();
 }
 template <int LOGD, int QC, int PS, int MT>
-static cudaError_t launch_xd_tma_t(const XdParams& p, const XtGeom& g, const CUtensorMap& tm, int grid, cudaStream_t s) {
-    return g_xd_tma_stages == 3 ? launch_xd_tma_n<LOGD, QC, PS, MT, 3>(p, g, tm, grid, s) : launch_xd_tma_n<LOGD, QC, PS, MT, 2>(p, g, tm, grid, s);
+static cudaError_t launch_xd_tma_t(const XdParams& p, const XtGeom& g, const CUtensorMap& tm, int grid, int stages, cudaStream_t s) {
+    return stages == 3 ? launch_xd_tma_n<LOGD, QC, PS, MT, 3>(p, g, tm, grid, s) : launch_xd_tma_n<LOGD, QC, PS, MT, 2>(p, g, tm, grid, s);
 }
-static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err, bool* f2) {
+static bool try_xd_tma(const XdParams& p, const KernelOpts& o, cudaStream_t s, cudaError_t* err, bool* f2) {
     const int D = p.D, PS = p.pfb_ps;
     if ((PS != 8 && PS != 10) || (D != 32 && D != 64) || !p.taps_host) { return false; }
     if (((uintptr_t)p.in & 15) != 0) { return false; }
@@ -974,7 +957,7 @@ static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err, bool
     memset(&g, 0, sizeof(g));
     g.org = org - sh;
     g.s = sh;
-    g.diag = g_xd_tma_diag;
+    g.diag = o.s1_diag;
     g.cj = (a0 - org) / D;                        // exact: a0 - org is a multiple of D
     long long jmin = g.cj;
     if (jmin & 1) { jmin -= 1; }
@@ -990,7 +973,7 @@ static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err, bool
     const int MT = (D == 32) ? 256 : 128;
     g.jend = (long long)g.cj + p.job[0].n_out;
     if (g.rows_tma < 8) { return false; }
-    // contiguous runs of whole tiles, one per persistent CTA (one per SM, or fewer: kernels_set_xd_tma_ctas leaves SMs free for
+    // contiguous runs of whole tiles, one per persistent CTA (one per SM, or fewer: KernelOpts::s1_ctas leaves SMs free for
     // the kernels of the other streams).  With the ÷4 epilogue every CTA but the first also filters the 32 outputs in front of
     // its run; the run is then 32 short of its tiles, and no CTA does more tiles than without the epilogue plus the halo.
     for (int v = 0; v < p.njobs; v++) {
@@ -998,7 +981,7 @@ static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err, bool
     }
     g.halo = g.f2 ? 32 : 0;
     int grid = num_sms();
-    if (g_xd_tma_ctas > 0 && g_xd_tma_ctas < grid) { grid = g_xd_tma_ctas; }
+    if (o.s1_ctas > 0 && o.s1_ctas < grid) { grid = o.s1_ctas; }
     const long long nblk = g.jend - jmin;
     const long long tiles_per_cta = cdiv(cdiv(nblk, grid) + g.halo, MT);
     g.run = (int)(tiles_per_cta * MT - g.halo);
@@ -1015,7 +998,8 @@ static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err, bool
     if (r != CUDA_SUCCESS) { return false; }
 #define XT_CASE(LD, Q, MTV)                                                                    \
     if (D == (1 << LD) && QC == Q) {                                                           \
-        *err = (PS == 10) ? launch_xd_tma_t<LD, Q, 10, MTV>(p, g, tm, grid, s) : launch_xd_tma_t<LD, Q, 8, MTV>(p, g, tm, grid, s); \
+        *err = (PS == 10) ? launch_xd_tma_t<LD, Q, 10, MTV>(p, g, tm, grid, o.s1_stages, s)                   \
+                          : launch_xd_tma_t<LD, Q, 8, MTV>(p, g, tm, grid, o.s1_stages, s);                    \
         *f2 = g.f2 != 0;                                                                       \
         return true;                                                                           \
     }
@@ -1025,14 +1009,15 @@ static bool try_xd_tma(const XdParams& p, cudaStream_t s, cudaError_t* err, bool
 }
 
 template <int FMT>
-static cudaError_t launch_xd_fmt(const XdParams& p, int variant, cudaStream_t s, int* nlaunch, bool* f2) {
+static cudaError_t launch_xd_fmt(const XdParams& p, int variant, const KernelOpts& o, cudaStream_t s, int* nlaunch, bool* tma, bool* f2) {
     int max_out = 0;
     for (int v = 0; v < p.njobs; v++) { max_out = p.job[v].n_out > max_out ? p.job[v].n_out : max_out; }
     if (max_out <= 0) { return cudaSuccess; }
     const int D = p.D;
     if (variant >= 7) {
         cudaError_t e = cudaSuccess;
-        if (variant >= 8 && FMT == FMT_CF32 && p.pfb_ps > 0 && try_xd_tma(p, s, &e, f2)) {
+        if (variant >= 8 && FMT == FMT_CF32 && p.pfb_ps > 0 && try_xd_tma(p, o, s, &e, f2)) {
+            *tma = true;
             if (nlaunch) { (*nlaunch)++; }
             return e;
         }
@@ -1046,7 +1031,7 @@ static cudaError_t launch_xd_fmt(const XdParams& p, int variant, cudaStream_t s,
         // per-VFO complex taps on cp.async tiles, 4-warp CTAs: 5 = double-buffered, one CTA per SM; anything else = one tile
         // buffer per CTA, three CTAs per SM (the retired 8- / 16-warp and single-buffer tile kernels map here)
         cudaError_t e = cudaSuccess;
-        if (try_xd_pipe<FMT>(p, s, &e, 4, variant != 5)) {
+        if (try_xd_pipe<FMT>(p, o, s, &e, 4, variant != 5)) {
             if (nlaunch) { (*nlaunch)++; }
             return e;
         }
@@ -1058,11 +1043,13 @@ static cudaError_t launch_xd_fmt(const XdParams& p, int variant, cudaStream_t s,
     return cudaGetLastError();
 }
 
-cudaError_t launch_xlate_decim(const XdParams& p, int fmt, int variant, cudaStream_t s, int* nlaunch, bool* f2) {
+cudaError_t launch_xlate_decim(const XdParams& p, int fmt, int variant, const KernelOpts& o, cudaStream_t s, int* nlaunch, bool* tma,
+                               bool* f2) {
+    *tma = false;
     *f2 = false;
-    if (fmt == FMT_CF32) { return launch_xd_fmt<FMT_CF32>(p, variant, s, nlaunch, f2); }
-    if (fmt == FMT_CS16) { return launch_xd_fmt<FMT_CS16>(p, variant, s, nlaunch, f2); }
-    return launch_xd_fmt<FMT_CS8>(p, variant, s, nlaunch, f2);
+    if (fmt == FMT_CF32) { return launch_xd_fmt<FMT_CF32>(p, variant, o, s, nlaunch, tma, f2); }
+    if (fmt == FMT_CS16) { return launch_xd_fmt<FMT_CS16>(p, variant, o, s, nlaunch, tma, f2); }
+    return launch_xd_fmt<FMT_CS8>(p, variant, o, s, nlaunch, tma, f2);
 }
 
 
@@ -1086,12 +1073,9 @@ cudaError_t launch_xd_edge(const XdParams& p, int fmt, cudaStream_t s, int* nlau
     return cudaGetLastError();
 }
 
-int g_tail_variant = 1;     // 0 = v0 kernels (operands through L1), 1 = shared-memory tiled kernels
-void kernels_set_tail_variant(int v) { g_tail_variant = v; }
-
-cudaError_t launch_fir_c(const FirParams& p, cudaStream_t s) {
+cudaError_t launch_fir_c(const FirParams& p, const KernelOpts& o, cudaStream_t s) {
     if (p.max_out <= 0 || p.njobs <= 0) { return cudaSuccess; }
-    if (g_tail_variant >= 1) {
+    if (o.tail_variant >= 1) {
         // all jobs of a batch share one kernel shape: pick by the first job, require the others to agree
         bool all_d1 = true, same_d = true;
         int maxT = 0, D0 = p.job[0].decim;
@@ -1128,9 +1112,9 @@ cudaError_t launch_fir_c(const FirParams& p, cudaStream_t s) {
     k_fir_c<<<grid, 256, 0, s>>>(p);
     return cudaGetLastError();
 }
-cudaError_t launch_poly(const PolyParams& p, cudaStream_t s) {
+cudaError_t launch_poly(const PolyParams& p, const KernelOpts& o, cudaStream_t s) {
     if (p.max_out <= 0 || p.njobs <= 0) { return cudaSuccess; }
-    if (g_tail_variant >= 1) {
+    if (o.tail_variant >= 1) {
         long long span_cap = 0, bank_floats = 0;
         for (int v = 0; v < p.njobs; v++) {
             long long sp = ((long long)PL2_THREADS * p.job[v].decim + p.job[v].interp - 1) / p.job[v].interp + p.job[v].tpp + 2;
@@ -1152,10 +1136,10 @@ cudaError_t launch_poly(const PolyParams& p, cudaStream_t s) {
     k_poly<<<grid, 256, 0, s>>>(p);
     return cudaGetLastError();
 }
-cudaError_t launch_quad(const QuadParams& p, cudaStream_t s) {
+cudaError_t launch_quad(const QuadParams& p, const KernelOpts& o, cudaStream_t s) {
     if (p.max_n <= 0 || p.njobs <= 0) { return cudaSuccess; }
     dim3 grid(cdiv(p.max_n, 256), p.njobs);
-    return launch_chain(k_quad, grid, dim3(256), 0, s, p);
+    return launch_chain(k_quad, grid, dim3(256), 0, o, s, p);
 }
 // resident CTAs of the fused tail per SM for a thread count and dynamic shared-memory size (registers included)
 // the opt-in shared-memory size of each k_tail_fused build only ever grows: the occupancy query and the launcher share it
@@ -1199,9 +1183,9 @@ cudaError_t launch_tail_fused(const FtParams& p, int max_slabs, int threads, siz
 #undef FT_LAUNCH
     return cudaGetLastError();
 }
-cudaError_t launch_fir_r(const FirRParams& p, cudaStream_t s) {
+cudaError_t launch_fir_r(const FirRParams& p, const KernelOpts& o, cudaStream_t s) {
     if (p.max_out <= 0 || p.njobs <= 0) { return cudaSuccess; }
-    if (g_tail_variant >= 1) {
+    if (o.tail_variant >= 1) {
         int maxT = 0;
         for (int v = 0; v < p.njobs; v++) { maxT = p.job[v].ntaps > maxT ? p.job[v].ntaps : maxT; }
         if (maxT <= TAIL_MAX_TAPS) {
@@ -1242,9 +1226,9 @@ cudaError_t launch_scale(const ScaleParams& p, cudaStream_t s) {
     k_scale<<<grid, 256, 0, s>>>(p);
     return cudaGetLastError();
 }
-cudaError_t launch_carry(const CarryParams& p, cudaStream_t s) {
+cudaError_t launch_carry(const CarryParams& p, const KernelOpts& o, cudaStream_t s) {
     if (p.njobs <= 0) { return cudaSuccess; }
-    return launch_chain(k_carry, dim3((unsigned)p.njobs), dim3(256), 0, s, p);
+    return launch_chain(k_carry, dim3((unsigned)p.njobs), dim3(256), 0, o, s, p);
 }
 
 bool fft_plan_uses_reg(const FftPlanDev& pl) {
@@ -1253,7 +1237,7 @@ bool fft_plan_uses_reg(const FftPlanDev& pl) {
 
 template <int FMT>
 static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const FftFrames& fr, float2* work, float* out_db, float2* out_raw,
-                                  cudaStream_t s, int* nlaunch, bool tables) {
+                                  const KernelOpts& o, cudaStream_t s, int* nlaunch, bool tables) {
     cudaError_t e;
     const int nbatch = fr.nbatch;
     if (pl.N1 == pl.N) {
@@ -1266,9 +1250,9 @@ static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const FftFrames& fr, flo
         return cudaGetLastError();
     }
     // two passes
-    if (g_fft_variant >= 1 && !out_raw && pl.tw_fine && pl.window_p && fft_plan_uses_reg(pl)) {
+    if (o.fft_variant >= 1 && !out_raw && pl.tw_fine && pl.window_p && fft_plan_uses_reg(pl)) {
         // register-resident column / row transforms (fft_reg.cuh)
-        // transforms per CTA: 8 (256 threads) or 4 (128 threads) -- kernels_set_fft_cta; DESIGN.md section 4 has the residency.
+        // transforms per CTA: 8 (256 threads) or 4 (128 threads) -- KernelOpts::fft_cta; DESIGN.md section 4 has the residency.
         // tables: + TW + N/TW float2 of twiddles in shared memory (pass 1), + TW (pass 2)
 #define FR_P1(RA, RB, CC)                                                                                      \
         do {                                                                                                   \
@@ -1298,7 +1282,7 @@ static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const FftFrames& fr, flo
                 k_fftr_p2<RA, RB, RR, false><<<dim3(pl.N1 / RR, nbatch), RR * FrGeom<RA, RB>::TP, sm, s>>>(pl, work, out_db); \
             }                                                                                                  \
         } while (0)
-        if (g_fft_cta == 4) {
+        if (o.fft_cta == 4) {
             if (pl.logN1 == 10) { FR_P1(32, 32, 4); } else if (pl.logN1 == 9) { FR_P1(16, 32, 4); } else { FR_P1(16, 16, 4); }
         }
         else {
@@ -1306,7 +1290,7 @@ static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const FftFrames& fr, flo
         }
         e = cudaGetLastError();
         if (e != cudaSuccess) { return e; }
-        if (g_fft_cta == 4) {
+        if (o.fft_cta == 4) {
             if (pl.logN2 == 10) { FR_P2(32, 32, 4); } else if (pl.logN2 == 9) { FR_P2(16, 32, 4); } else { FR_P2(16, 16, 4); }
         }
         else {
@@ -1344,7 +1328,7 @@ static cudaError_t launch_fft_fmt(const FftPlanDev& pl, const FftFrames& fr, flo
 // gridDim.y holds a batch's frame index, so a batch of more frames is launched in slices of at most this many
 #define FFT_MAX_GRID_Y 65535
 cudaError_t launch_fft_frames(const FftPlanDev& pl, const FftFrames& fr, int fmt, float2* work, float* out_db,
-                              float2* out_raw, cudaStream_t s, int* nlaunch, bool tables) {
+                              float2* out_raw, const KernelOpts& o, cudaStream_t s, int* nlaunch, bool tables) {
     const int bps = fmt == FMT_CF32 ? 8 : (fmt == FMT_CS16 ? 4 : 2);
     for (int f0 = 0; f0 < fr.nbatch; f0 += FFT_MAX_GRID_Y) {
         // slice 0 keeps the staged part of its first frame; a later slice's first frame lies wholly in the chunk
@@ -1359,17 +1343,17 @@ cudaError_t launch_fft_frames(const FftPlanDev& pl, const FftFrames& fr, int fmt
         float* const db = out_db ? out_db + (size_t)f0 * pl.N : nullptr;
         float2* const raw = out_raw ? out_raw + (size_t)f0 * pl.N : nullptr;
         cudaError_t e;
-        if (fmt == FMT_CF32) { e = launch_fft_fmt<FMT_CF32>(pl, sl, w, db, raw, s, nlaunch, tables); }
-        else if (fmt == FMT_CS16) { e = launch_fft_fmt<FMT_CS16>(pl, sl, w, db, raw, s, nlaunch, tables); }
-        else { e = launch_fft_fmt<FMT_CS8>(pl, sl, w, db, raw, s, nlaunch, tables); }
+        if (fmt == FMT_CF32) { e = launch_fft_fmt<FMT_CF32>(pl, sl, w, db, raw, o, s, nlaunch, tables); }
+        else if (fmt == FMT_CS16) { e = launch_fft_fmt<FMT_CS16>(pl, sl, w, db, raw, o, s, nlaunch, tables); }
+        else { e = launch_fft_fmt<FMT_CS8>(pl, sl, w, db, raw, o, s, nlaunch, tables); }
         if (e != cudaSuccess) { return e; }
     }
     return cudaSuccess;
 }
 cudaError_t launch_fft_frame(const FftPlanDev& pl, const void* src, int fmt, float2* work, float* out_db,
-                             float2* out_raw, cudaStream_t s, int* nlaunch) {
+                             float2* out_raw, const KernelOpts& o, cudaStream_t s, int* nlaunch) {
     const FftFrames fr{ src, nullptr, 0, 0, 1 };
-    return launch_fft_frames(pl, fr, fmt, work, out_db, out_raw, s, nlaunch, true);
+    return launch_fft_frames(pl, fr, fmt, work, out_db, out_raw, o, s, nlaunch, true);
 }
 
 cudaError_t launch_convert_cf32(const void* src, int fmt, float2* dst, int n, float scale, cudaStream_t s) {

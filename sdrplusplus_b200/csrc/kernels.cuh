@@ -7,6 +7,20 @@
 
 #define B200_BATCH 16
 
+// ---- launch-time kernel choices of one handle (b200_fe_set_option); every launcher with a choice takes them explicitly ----
+#define PDL_DEFAULT 2
+int kernels_pdl_default();      // env B200_PDL, read once per process, else PDL_DEFAULT
+struct KernelOpts {
+    int tail_variant = 1;       // 0 = one thread per output (operands through L1), 1 = shared-memory tiled kernels
+    int fft_variant = 1;        // 1 = register-resident four-step passes where they apply, 0 = shared-memory radix-8 passes
+    int fft_cta = 8;            // column / row transforms per CTA of the register-resident passes: 8 or 4
+    int pdl = kernels_pdl_default();    // programmatic dependent launch of the chain kernels: 0 off, 1 always, 2 small grids only
+    int s1_mt = 0;              // tile of k_xd_pipe in outputs (rounded down to a multiple of 128), 0 = automatic
+    int s1_stages = 2;          // ring depth of k_xd_tma, 2 or 3: 2 leaves a third of the SM's shared memory to the other streams
+    int s1_ctas = 0;            // persistent CTAs of k_xd_tma, 0 = one per SM
+    int s1_diag = 0;            // XtGeom::diag, measurement only: 1 = load the tiles, do not filter; 2 = filter, do not load
+};
+
 // ---- sample formats (must match include/b200dsp.h) ----
 enum { FMT_CF32 = 0, FMT_CS16 = 1, FMT_CS8 = 2 };
 
@@ -84,7 +98,7 @@ struct DfrParams {
 };
 
 bool dfir_reg_supported(int D, int T);
-cudaError_t launch_dfir_reg(const DfrParams& p, int D, int T, cudaStream_t s);
+cudaError_t launch_dfir_reg(const DfrParams& p, int D, int T, const KernelOpts& o, cudaStream_t s);
 
 // ---- polyphase rational resampler (PolyphaseResampler::process, polyphase_resampler.h:69-99) ----
 // output m: t = phase0 + m*decim; off = offset0 + t/interp; ph = t%interp;
@@ -100,7 +114,7 @@ struct PolyJob {
 struct PolyParams { int njobs; int max_out; PolyJob job[B200_BATCH]; };
 // register-window versions of the output-rate stages (tails_reg.cuh)
 bool poly_reg_supported(int interp, int decim);
-cudaError_t launch_poly_reg(const PolyParams& p, cudaStream_t s);           // every job: the same (interp, decim)
+cudaError_t launch_poly_reg(const PolyParams& p, const KernelOpts& o, cudaStream_t s);     // every job: the same (interp, decim)
 
 // ---- FM discriminator (Quadrature::process, quadrature.h:39-46) ----
 struct QuadJob {
@@ -318,10 +332,6 @@ struct RdsJob {
 struct RdsParams { int njobs; int pad; RdsJob job[B200_BATCH]; };
 cudaError_t launch_rds_demod(const RdsParams& p, cudaStream_t s);
 
-// programmatic dependent launch for the chain kernels behind stage 1 (kernels.cu: launch_chain); env B200_PDL, option "pdl"
-int kernels_pdl();
-void kernels_set_pdl(int on);
-
 // ---- noise_reduction::PowerSquelch at the VFO output (stereo.cuh) ----
 #define SQ_MAXPARTS 256
 struct SqJob { const float2* in; float2* out; float* partial; int n; float level; };
@@ -378,19 +388,21 @@ struct FftPlanDev {
 };
 
 // launch wrappers (return cudaGetLastError())
-// *f2 = true when the launch ran the ÷4 epilogue of the jobs that carry one (k_xd_tma); false: every job stored `out`
-cudaError_t launch_xlate_decim(const XdParams& p, int fmt, int variant, cudaStream_t s, int* nlaunch, bool* f2);
+// *tma = true when the launch ran k_xd_tma; *f2 = true when it ran the ÷4 epilogue of the jobs that carry one (k_xd_tma);
+// false: every job stored `out`
+cudaError_t launch_xlate_decim(const XdParams& p, int fmt, int variant, const KernelOpts& o, cudaStream_t s, int* nlaunch, bool* tma,
+                               bool* f2);
 cudaError_t launch_xd_edge(const XdParams& p, int fmt, cudaStream_t s, int* nlaunch);
-cudaError_t launch_fir_c(const FirParams& p, cudaStream_t s);
-cudaError_t launch_fir_reg(const FirParams& p, cudaStream_t s);            // every job: decimation 1
-cudaError_t launch_firr_reg(const FirRParams& p, cudaStream_t s);
-cudaError_t launch_poly(const PolyParams& p, cudaStream_t s);
-cudaError_t launch_quad(const QuadParams& p, cudaStream_t s);
-cudaError_t launch_fir_r(const FirRParams& p, cudaStream_t s);
+cudaError_t launch_fir_c(const FirParams& p, const KernelOpts& o, cudaStream_t s);
+cudaError_t launch_fir_reg(const FirParams& p, const KernelOpts& o, cudaStream_t s);      // every job: decimation 1
+cudaError_t launch_firr_reg(const FirRParams& p, const KernelOpts& o, cudaStream_t s);
+cudaError_t launch_poly(const PolyParams& p, const KernelOpts& o, cudaStream_t s);
+cudaError_t launch_quad(const QuadParams& p, const KernelOpts& o, cudaStream_t s);
+cudaError_t launch_fir_r(const FirRParams& p, const KernelOpts& o, cudaStream_t s);
 cudaError_t launch_seq(const SeqParams& p, cudaStream_t s);
 cudaError_t launch_m2s(const M2SParams& p, cudaStream_t s);
 cudaError_t launch_scale(const ScaleParams& p, cudaStream_t s);
-cudaError_t launch_carry(const CarryParams& p, cudaStream_t s);
+cudaError_t launch_carry(const CarryParams& p, const KernelOpts& o, cudaStream_t s);
 // Where a batch of frames comes from: frame f's sample n is chunk[f * stride + n - split] (format fmt, index in samples).
 // split > 0 only for a frame that began in earlier chunks: its first split samples were staged, in the same format, at
 // pre[0 .. split), and chunk points at the first sample of this chunk.
@@ -403,11 +415,11 @@ struct FftFrames {
 };
 // src: nz samples of format fmt (chunk data), read directly; out_db: N floats; work: N float2 scratch
 cudaError_t launch_fft_frame(const FftPlanDev& pl, const void* src, int fmt, float2* work, float* out_db,
-                             float2* out_raw, cudaStream_t s, int* nlaunch);
+                             float2* out_raw, const KernelOpts& o, cudaStream_t s, int* nlaunch);
 // fr.nbatch frames in one launch pair; work: nbatch*N float2, out_db: nbatch*N.  tables: the register passes stage their
 // twiddle tables in shared memory and read the window as vectors (same values, same output bits); false = global gathers
 cudaError_t launch_fft_frames(const FftPlanDev& pl, const FftFrames& fr, int fmt, float2* work, float* out_db,
-                              float2* out_raw, cudaStream_t s, int* nlaunch, bool tables);
+                              float2* out_raw, const KernelOpts& o, cudaStream_t s, int* nlaunch, bool tables);
 // the register passes serve this plan (pass-1 window order: window_p)
 bool fft_plan_uses_reg(const FftPlanDev& pl);
 // IQFrontEnd pre-processing at the input rate: DC blocker + conjugate (preproc.cuh)
@@ -447,11 +459,3 @@ cudaError_t launch_index_max(const float* in, long long n, float* out_val, cudaS
 cudaError_t launch_zoom_hold_tbl(const float* line, const int* start, const int* len, int out_size, float* out,
                                  float* hold, float hold_speed, cudaStream_t s);
 int kernels_max_smem_optin();
-void kernels_set_tail_variant(int v);
-void kernels_set_fft_variant(int v);
-void kernels_set_xd_tma_ctas(int v);      // persistent CTAs of the TMA stage 1 (0 = one per SM)
-void kernels_set_fft_cta(int v);          // transforms per CTA of the register FFT passes (8 or 4)
-void kernels_set_xd_tile(int mt);     // 0 = automatic
-void kernels_set_xd_tma_diag(int v);      // measurement only: 1 = load the tiles, do not filter; 2 = filter, do not load
-void kernels_set_xd_tma_stages(int n);   // ring depth of the TMA stage 1 (2 or 3)
-void kernels_set_xd_cps(int v);       // cap on stage-1 CTAs per SM, 0 = automatic

@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(TR_THREADS) k_poly_reg(const __grid_constant__
     }
 }
 template <int L, int M>
-static cudaError_t launch_poly_reg_t(const PolyParams& p, int max_tpp, cudaStream_t s) {
+static cudaError_t launch_poly_reg_t(const PolyParams& p, int max_tpp, const KernelOpts& o, cudaStream_t s) {
     using G = PolyGeom<L, M>;
     static_assert(TR_THREADS == PR_SPLIT * 32, "one warp per tap range");
     const size_t nx = (size_t)(PR_PER - 1) * M + G::W + max_tpp;
@@ -133,22 +133,22 @@ static cudaError_t launch_poly_reg_t(const PolyParams& p, int max_tpp, cudaStrea
     if (e != cudaSuccess) { return e; }
     const int periods = (p.max_out + L - 1) / L + 1;
     dim3 grid((unsigned)((periods + PR_PER - 1) / PR_PER), (unsigned)p.njobs);
-    return launch_chain(k_poly_reg<L, M>, grid, dim3(TR_THREADS), smem, s, p);
+    return launch_chain(k_poly_reg<L, M>, grid, dim3(TR_THREADS), smem, o, s, p);
 }
 bool poly_reg_supported(int L, int M) {
     return (L == 16 && M == 25) || (L == 5 && M == 6) || (L == 2 && M == 3) || (L == 4 && M == 5) || (L == 2 && M == 5);
 }
 // every job of p: the same (interp, decim)
-cudaError_t launch_poly_reg(const PolyParams& p, cudaStream_t s) {
+cudaError_t launch_poly_reg(const PolyParams& p, const KernelOpts& o, cudaStream_t s) {
     if (p.njobs <= 0 || p.max_out <= 0) { return cudaSuccess; }
     const int L = p.job[0].interp, M = p.job[0].decim;
     int max_tpp = 0;
     for (int v = 0; v < p.njobs; v++) { max_tpp = p.job[v].tpp > max_tpp ? p.job[v].tpp : max_tpp; }
-    if (L == 16 && M == 25) { return launch_poly_reg_t<16, 25>(p, max_tpp, s); }
-    if (L == 5 && M == 6) { return launch_poly_reg_t<5, 6>(p, max_tpp, s); }
-    if (L == 2 && M == 3) { return launch_poly_reg_t<2, 3>(p, max_tpp, s); }
-    if (L == 4 && M == 5) { return launch_poly_reg_t<4, 5>(p, max_tpp, s); }
-    if (L == 2 && M == 5) { return launch_poly_reg_t<2, 5>(p, max_tpp, s); }
+    if (L == 16 && M == 25) { return launch_poly_reg_t<16, 25>(p, max_tpp, o, s); }
+    if (L == 5 && M == 6) { return launch_poly_reg_t<5, 6>(p, max_tpp, o, s); }
+    if (L == 2 && M == 3) { return launch_poly_reg_t<2, 3>(p, max_tpp, o, s); }
+    if (L == 4 && M == 5) { return launch_poly_reg_t<4, 5>(p, max_tpp, o, s); }
+    if (L == 2 && M == 5) { return launch_poly_reg_t<2, 5>(p, max_tpp, o, s); }
     return cudaErrorInvalidValue;
 }
 
@@ -245,7 +245,7 @@ __global__ void __launch_bounds__(TR_THREADS) k_fir_reg(const __grid_constant__ 
     }
 }
 // every job: decimation 1
-cudaError_t launch_fir_reg(const FirParams& p, cudaStream_t s) {
+cudaError_t launch_fir_reg(const FirParams& p, const KernelOpts& o, cudaStream_t s) {
     if (p.njobs <= 0 || p.max_out <= 0) { return cudaSuccess; }
     int maxT = 0;
     for (int v = 0; v < p.njobs; v++) { maxT = p.job[v].ntaps > maxT ? p.job[v].ntaps : maxT; }
@@ -255,7 +255,7 @@ cudaError_t launch_fir_reg(const FirParams& p, cudaStream_t s) {
     cudaError_t e = set_smem(k_fir_reg, smem);
     if (e != cudaSuccess) { return e; }
     dim3 grid((unsigned)((p.max_out + TS_TILE - 1) / TS_TILE), (unsigned)p.njobs);
-    return launch_chain(k_fir_reg, grid, dim3(TR_THREADS), smem, s, p);
+    return launch_chain(k_fir_reg, grid, dim3(TR_THREADS), smem, o, s, p);
 }
 
 // ------------------------------------------------------------------------------------------------ real FIR (+ mono -> stereo)
@@ -357,7 +357,7 @@ __global__ void __launch_bounds__(TR_THREADS) k_firr_reg(const __grid_constant__
         }
     }
 }
-cudaError_t launch_firr_reg(const FirRParams& p, cudaStream_t s) {
+cudaError_t launch_firr_reg(const FirRParams& p, const KernelOpts& o, cudaStream_t s) {
     if (p.njobs <= 0 || p.max_out <= 0) { return cudaSuccess; }
     int maxT = 0;
     for (int v = 0; v < p.njobs; v++) { maxT = p.job[v].ntaps > maxT ? p.job[v].ntaps : maxT; }
@@ -369,5 +369,5 @@ cudaError_t launch_firr_reg(const FirRParams& p, cudaStream_t s) {
     cudaError_t e = set_smem(k_firr_reg, smem);
     if (e != cudaSuccess) { return e; }
     dim3 grid((unsigned)((p.max_out + TS_TILE - 1) / TS_TILE), (unsigned)p.njobs);
-    return launch_chain(k_firr_reg, grid, dim3(TR_THREADS), smem, s, p);
+    return launch_chain(k_firr_reg, grid, dim3(TR_THREADS), smem, o, s, p);
 }

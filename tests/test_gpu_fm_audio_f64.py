@@ -35,7 +35,7 @@ vfo_settings_oracle.py (a high-pass switched off keeps its delay line; de-emphas
 In situ stage 1's a-priori bound dominates; the fitted gain |g - 1| < 2e-6 and the edge-against-interior ratio <= 4
 (f64_ref._gate_vfo) carry the fine sensitivity there, the stand-alone blocks carry it for the kernels themselves.
 Each front-end option set profiles one chunk and asserts that the kernels behind stage 1 that ran are those the routing
-mirror names; every case sets the process-wide tail variant ("tails") itself and puts the default back afterwards.
+mirror names; every case sets its options, the tail variant ("tails") among them, on its own front end.
 No tolerance here is fitted to a run.
 """
 import math
@@ -510,23 +510,11 @@ def v_reference(oracle, v_input):
 
 
 def _front_end(sb, fs, max_chunk, opts):
-    """a front end with the case's options.  "tails" selects the process-wide tail variant (kernels_set_tail_variant), which
-    a new front end does not reset: every case sets it, the default (2) included, before its VFOs are added."""
+    """a front end with the case's options, set before its VFOs are added"""
     fe = sb.FrontEnd(fs, max_chunk)
-    fe.set_option("tails", opts.get("tails", 2))
     for k, v in opts.items():
-        if k != "tails":
-            fe.set_option(k, v)
+        fe.set_option(k, v)
     return fe
-
-
-def _restore_tails(sb):
-    """put the process-wide tail variant back to the default for the modules that run after this one"""
-    fe = sb.FrontEnd(FS_V, 1024)
-    try:
-        fe.set_option("tails", 2)
-    finally:
-        fe.close()
 
 
 TAIL_KERNELS = {"k_quad", "k_firr_reg", "k_fir_r2", "k_fir_r", "k_poly_reg", "k_poly2", "k_poly", "k_fir_reg", "k_fir_c2",
@@ -599,7 +587,6 @@ def test_fm_vfos_in_front_end_vs_float64(sb, oracle, v_input, v_reference, repor
         hits = fe.stat("graph_hits")
     finally:
         fe.close()
-        _restore_tails(sb)
     res = []
     for k, vid in enumerate(ids):
         c = vs[k][0]
@@ -667,7 +654,6 @@ def test_wfm_vfos_behind_tma_stage1_100msps(sb, oracle, report):
         fused = fe.stat("fused_chains")
     finally:
         fe.close()
-        _restore_tails(sb)
     assert tma > 0 and fused == 0
     xr = x.astype(np.complex128)
     res = []
@@ -738,7 +724,6 @@ def test_changes_at_chunk_boundaries(sb, oracle, report):
             pos += m
     finally:
         fe.close()
-        _restore_tails(sb)
     xr = x.astype(np.complex128)
     res = {}
     for name, vid, c in zip(("wfm_af", "nfm_af"), ids, cfgs):

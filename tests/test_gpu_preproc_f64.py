@@ -665,9 +665,6 @@ def _s1_run(sb, fs, ratio, offs, chunks, fmt, scale, decim=1, dc=True, conj=True
             for v in ids:
                 got[v].append(outs[v])
     finally:
-        fe.set_option("s1_mt", 0)
-        fe.set_option("s1_stages", 2)
-        fe.set_option("s1_ctas", 0)
         fe.close()
     return [got[v] for v in ids], tap, tma, f2
 

@@ -128,8 +128,6 @@ def test_records_and_audio_equal_the_two_vfo_way(sb, report, build):
     outs, _ = fe.process_chunks(x, chunk)
     fused = fe.stat("fused_chains")
     fe.close()
-    if "tails" in opts:
-        sb.FrontEnd(FS, chunk).set_option("tails", 2)         # the tail kernel build is process-wide: back to the default
     if opts.get("ft_regall") == 0:
         assert fused >= 2                                     # the parent's discriminator ran inside k_tail_fused
     report["rds_bound_" + "_".join(str(b) for b in build[:4]) + "_" + str(sorted(opts.items()))] = {"symbols": int(outs[vr][0].size)}

@@ -11,8 +11,7 @@ import numpy as np
 import pytest
 
 from f64_ref import plan_of
-from test_gpu_stage1_f64 import (CASES, CF32, CS16, FS, PS10M, Run, _gate_parts, _restore_process_wide, fir_offsets,  # noqa: F401
-                                 sb)
+from test_gpu_stage1_f64 import CASES, CF32, CS16, FS, PS10M, Run, _gate_parts, fir_offsets, sb  # noqa: F401
 
 F2 = (4, 27)
 
@@ -141,7 +140,6 @@ def _run_chunks(sb, r):
             for vid in ids:
                 got[vid].append(outs[vid])
     finally:
-        _restore_process_wide(fe)
         fe.close()
     return [got[vid] for vid in ids], tma, f2
 

@@ -50,8 +50,6 @@ def _lines(sb, chunks, fs, size, rate, v, decim=1, scales=None, cta=None):
         launches.append(fe.launch_count() - l0)
         if ln.size:
             lines.append(ln)
-    if cta:
-        fe.set_option("fft_cta", 8)          # process-wide: back to the default
     fe.close()
     return (np.concatenate(lines) if lines else np.empty((0, size), np.float32)), launches
 

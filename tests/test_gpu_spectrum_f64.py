@@ -591,8 +591,6 @@ def _run_fe(sb, case, chunks, scales, fft=True, taps=False):
             if taps:
                 tap.append(outs[tid])
     finally:
-        fe.set_option("fft_cta", 8)          # process-wide options: back to the defaults
-        fe.set_option("fft", 1)
         fe.close()
     return [(l[0] if len(l) == 1 else np.concatenate(l)) if l else np.empty((0, 1), np.float32) for l in lines], launches, tap
 

@@ -443,13 +443,6 @@ def sb():
     return m
 
 
-def _restore_process_wide(fe):
-    # s1_mt, s1_stages and s1_ctas are process-wide kernel settings: put back the defaults
-    fe.set_option("s1_mt", 0)
-    fe.set_option("s1_stages", 2)
-    fe.set_option("s1_ctas", 0)
-
-
 def _run_front_end(sb, r, chunks=None):
     fe = sb.FrontEnd(FS, max(max(r.sched), 1))
     try:
@@ -474,7 +467,6 @@ def _run_front_end(sb, r, chunks=None):
                 got[vid].append(outs[vid])
         tma = fe.stat("s1_tma_launches") - t0
     finally:
-        _restore_process_wide(fe)
         fe.close()
     return [got[vid] for vid in ids], tma
 

@@ -318,19 +318,9 @@ def fe_input(fs, vs, n, seed):
 
 def _front_end(sb, fs, max_chunk, opts):
     fe = sb.FrontEnd(fs, max_chunk)
-    fe.set_option("tails", opts.get("tails", 2))
     for k, v in opts.items():
-        if k != "tails":
-            fe.set_option(k, v)
+        fe.set_option(k, v)
     return fe
-
-
-def _restore_tails(sb):
-    fe = sb.FrontEnd(FS_V, 1024)
-    try:
-        fe.set_option("tails", 2)
-    finally:
-        fe.close()
 
 
 def run_front_end(sb, fs, cfgs, x, sched, opts=None, levels=None, reset_at=None):
@@ -356,7 +346,6 @@ def run_front_end(sb, fs, cfgs, x, sched, opts=None, levels=None, reset_at=None)
         return [got[vid] for vid in ids], fe.stat("graph_hits")
     finally:
         fe.close()
-        _restore_tails(sb)
 
 
 V_OPTIONS = [{}, {"ft_regall": 0}, {"tails": 1, "ft_prereg": 0}, {"tails": 0, "ft_prereg": 0}, {"graph": 0}]
